@@ -68,5 +68,17 @@ def test_argument_validation_without_a_gpu():
     assert L.b2_allreduce_gather(None, ctypes.c_void_p(4096), 20, segs, 2, 0, 1.0, 0, None) == N.B2_EINVAL
     assert b"does not continue" in L.b2_last_error()
     assert L.b2_allreduce_gather(None, ctypes.c_void_p(4096), 20, segs, N.B2_MAX_SEGMENTS + 1, 0, 1.0, 0, None) == N.B2_EINVAL
+    assert b"need 1..128 segments (got 129)" in L.b2_last_error()
+    assert L.b2_allreduce_gather(None, ctypes.c_void_p(4096), 20, segs, 0, 0, 1.0, 0, None) == N.B2_EINVAL
+    assert b"need 1..128 segments (got 0)" in L.b2_last_error()
+    for bad in ((8192, 8, 20), (8192, 10, 10), (None, 10, 20)):  # overlaps segment 0 / empty / null source
+        segs[1].src, segs[1].begin, segs[1].end = bad
+        assert L.b2_allreduce_gather(None, ctypes.c_void_p(4096), 20, segs, 2, 0, 1.0, 0, None) == N.B2_EINVAL, bad
+        assert b"segment 1 does not continue the bucket at element 10" in L.b2_last_error(), bad
+    segs[1].src, segs[1].begin, segs[1].end = 8192, 10, 20
+    for n in (19, 21):  # the table covers more / fewer elements than the bucket has
+        assert L.b2_allreduce_gather(None, ctypes.c_void_p(4096), n, segs, 2, 0, 1.0, 0, None) == N.B2_EINVAL, n
+        assert f"segments cover 20 elements, bucket has {n}".encode() in L.b2_last_error(), n
+    assert L.b2_allreduce_gather(None, None, 0, None, 0, 0, 1.0, 0, None) == N.B2_OK  # n_elems == 0: a no-op, table unread
     assert L.b2_comm_caps(None) == N.B2_EINVAL and L.b2_comm_last_algo(None) == N.B2_EINVAL
     assert L.b2_comm_set_param(None, b"max_ctas", 1) == N.B2_EINVAL

@@ -7,12 +7,11 @@ import pytest
 import torch
 
 import oracle
-from tests._util import assert_bits_equal, assert_nvls_result, make_inputs
+from tests._util import (GUARD, MODES, POISON, WIRE, World, assert_bits_equal, assert_guards_intact, assert_nvls_result, make_inputs,
+                         to_dev, to_host)
 
 pytestmark = pytest.mark.gpu
 
-MODES = {"f32_wire_bf16": oracle.B2O_F32_WIRE_BF16, "f32": oracle.B2O_F32, "bf16": oracle.B2O_BF16}
-WIRE = {"f32_wire_bf16": "bf16", "f32": "f32", "bf16": "bf16"}
 SIZES = [1, 7, 8, 9, 1023, 1024, 1025, 4099, 32771, (1 << 18) + 5]
 
 
@@ -24,66 +23,33 @@ def _devices(world, cuda_count, spread):
     return [0] * world
 
 
-class World:
-    def __init__(self, devices, stage_mb=8, timeout_s=10.0):
-        from torchx_b200.ddp import Communicator
-
-        self.comms = Communicator.create_local(devices, stage_mb=stage_mb)
-        self.streams = [torch.cuda.Stream(device=d) for d in devices]
-        same_device = len(set(devices)) == 1
-        for c in self.comms:
-            c.set_timeout(timeout_s)
-            if same_device:  # all kernels must be co-resident on one GPU: W ranks x grid <= #SMs (1 CTA per SM)
-                c.set_max_ctas(max(1, 128 // len(devices)))
-
-    def run(self, fn):
-        """fn(rank, comm, stream) launches that rank's work; then wait for all and check health."""
-        for r, (c, s) in enumerate(zip(self.comms, self.streams)):
-            fn(r, c, s)
-        for s in self.streams:
-            s.synchronize()
-        for c in self.comms:
-            c.check()
-
-    def close(self):
-        for c in self.comms:
-            c.close()
-
-
-def _to_dev(x, mode, device):
-    if mode == "bf16":
-        bits = oracle.f32_to_bf16_bits(x)
-        return torch.from_numpy(bits.view(np.int16).copy()).to(f"cuda:{device}").view(torch.bfloat16), bits
-    return torch.from_numpy(x.copy()).to(f"cuda:{device}"), x
-
-
-def _to_host(t, mode):
-    if mode == "bf16":
-        return t.view(torch.int16).cpu().numpy().view(np.uint16)
-    return t.cpu().numpy()
-
-
 def _check_allreduce(world_obj, n, mode, algo, kind, seed, offset=0):
+    """Each rank's tensor is elements [offset, offset + n) of an allocation of n + offset + GUARD elements; the elements
+    around it hold POISON and must come back unchanged."""
     W = len(world_obj.comms)
     xs = make_inputs(W, n + offset, seed, kind)
-    tens, host = [], []
+    full, tens, host, before = [], [], [], []
     for r, c in enumerate(world_obj.comms):
-        t, h = _to_dev(xs[r], mode, c.device)
-        tens.append(t[offset:])
-        host.append(h[offset:])
+        t, h = to_dev(np.concatenate([xs[r], np.full(GUARD, POISON)]), mode, c.device)
+        full.append(t)
+        tens.append(t[offset:offset + n])
+        host.append(h[offset:offset + n])
+        before.append(h)
     scale = 1.0 / W
     world_obj.run(lambda r, c, s: c.allreduce_(tens[r], scale=scale, wire=WIRE[mode], algo=algo, stream=s))
     what = f"W={W} n={n} mode={mode} algo={algo} kind={kind}"
+    for r in range(W):
+        assert_guards_intact(to_host(full[r], mode), before[r], offset, offset + n, f"{what} rank={r}")
     ran_nvls = world_obj.comms[0].last_algo == "nvls"
     if ran_nvls and kind != "onehot":  # onehot: one non-zero term per element - exact on every path
         # the switch's own arithmetic (tools/nvls_probe.py, DESIGN.md 2.4): within one bf16 ulp of the exact sum
-        stats = [assert_nvls_result(_to_host(tens[r], mode), host, scale, MODES[mode], f"{what} rank={r}") for r in range(W)]
+        stats = [assert_nvls_result(to_host(tens[r], mode), host, scale, MODES[mode], f"{what} rank={r}") for r in range(W)]
         for r in range(1, W):  # every rank holds the SAME bits (one reduction per element, replicated by the switch)
-            assert_bits_equal(_to_host(tens[r], mode), _to_host(tens[0], mode), f"{what}: rank {r} vs rank 0")
+            assert_bits_equal(to_host(tens[r], mode), to_host(tens[0], mode), f"{what}: rank {r} vs rank 0")
         return stats[0]
     want = oracle.allreduce(MODES[mode], host, scale)
     for r in range(W):
-        assert_bits_equal(_to_host(tens[r], mode), want, f"{what} rank={r}")
+        assert_bits_equal(to_host(tens[r], mode), want, f"{what} rank={r}")
     return None
 
 
@@ -95,13 +61,16 @@ def test_local_pass_matches_oracle(mode):
         for kind in ("randn", "special"):
             for offset in (0, 1):
                 x = make_inputs(1, n + offset, 7, kind)[0]
-                t, h = _to_dev(x, mode, 0)
+                t, h = to_dev(np.concatenate([x, np.full(GUARD, POISON)]), mode, 0)
                 for scale in (1.0, 0.125, 1.0 / 3.0):
-                    tt = t.clone()[offset:]
+                    full = t.clone()
+                    tt = full[offset:offset + n]
                     local_pass_(tt, scale=scale, wire=WIRE[mode])
                     torch.cuda.synchronize()
-                    want = oracle.allreduce(MODES[mode], [h[offset:]], scale)
-                    assert_bits_equal(_to_host(tt, mode), want, f"local n={n} mode={mode} scale={scale} off={offset}")
+                    what = f"local n={n} mode={mode} scale={scale} off={offset}"
+                    assert_guards_intact(to_host(full, mode), h, offset, offset + n, what)
+                    want = oracle.allreduce(MODES[mode], [h[offset:offset + n]], scale)
+                    assert_bits_equal(to_host(tt, mode), want, what)
 
 
 @pytest.mark.parametrize("world", [2, 3, 4, 8])
@@ -113,6 +82,7 @@ def test_allreduce_matches_oracle_one_device(world, mode, algo):
         for i, n in enumerate(SIZES):
             _check_allreduce(w, n, mode, algo, "randn" if i % 2 == 0 else "special", seed=i)
         _check_allreduce(w, 4099, mode, algo, "randn", seed=99, offset=1)  # misaligned base pointer
+        _check_allreduce(w, 4099, mode, algo, "nanbits", seed=11)  # NaN payloads, the sentinel word, +-inf
         _check_allreduce(w, 1 << 12, mode, algo, "onehot", seed=0)
         _check_allreduce(w, 1 << 12, mode, algo, "ints", seed=0)
     finally:

@@ -259,6 +259,80 @@ def test_zero_copy_bucket_fill_equals_copy_in(zero_copy):
             c.close()
 
 
+def _grad_bits(m):
+    """Flat gradients as bit patterns: bf16 as uint16, fp32 as float32."""
+    g = torch.cat([p.grad.reshape(-1) for p in m.parameters()])
+    return g.view(torch.int16).cpu().numpy().view(np.uint16) if g.dtype == torch.bfloat16 else g.cpu().numpy()
+
+
+def _check_ddp_against_twins(W, make, mode, steps=2, **kw):
+    """W ranks of DistributedDataParallel(make()) against the oracle on the gradients of un-synced twins; returns rank 0's
+    DistributedDataParallel (for its bucket counters).  One warm-up backward per rank under no_sync() first, so that no
+    first-use allocation happens on a rank's stream while a peer's kernel spins."""
+    from torchx_b200.ddp import Communicator, DistributedDataParallel
+
+    comms = Communicator.create_local([0] * W, stage_mb=8)
+    try:
+        streams = [torch.cuda.Stream() for _ in range(W)]
+        ddps = []
+        for r in range(W):
+            comms[r].set_timeout(20.0)
+            comms[r].set_max_ctas(4)
+            with torch.cuda.stream(streams[r]):
+                ddps.append(DistributedDataParallel(make(), comms[r], **kw))
+        torch.cuda.synchronize()
+        dtype = next(ddps[0].parameters()).dtype
+        for r in range(W):
+            with torch.cuda.stream(streams[r]), ddps[r].no_sync():
+                ddps[r](torch.zeros(8, 64, device="cuda", dtype=dtype)).square().mean().backward()
+                ddps[r].zero_grad(set_to_none=True)
+        torch.cuda.synchronize()
+        for step in range(steps):
+            xs = [torch.randn(8, 64, device="cuda", generator=torch.Generator("cuda").manual_seed(11 * step + r)).to(dtype) for r in range(W)]
+            local = []
+            for r in range(W):
+                twin = make()
+                twin.load_state_dict(ddps[r].module.state_dict())
+                twin(xs[r]).square().mean().backward()
+                local.append(_grad_bits(twin))
+            for r in range(W):
+                with torch.cuda.stream(streams[r]):
+                    ddps[r].zero_grad(set_to_none=True)
+                    ddps[r](xs[r]).square().mean().backward()
+            torch.cuda.synchronize()
+            for c in comms:
+                c.check()
+            want = oracle.allreduce(mode, local, 1.0 / W)
+            for r in range(W):
+                assert_bits_equal(_grad_bits(ddps[r].module), want, f"step {step} rank {r}")
+        return ddps[0]
+    finally:
+        for c in comms:
+            c.close()
+
+
+@pytest.mark.parametrize("W", [2, 4])
+@pytest.mark.parametrize("algo", ["oneshot", "twoshot", "twoshot_pipe", "twoshot_ll"])
+def test_bf16_parameters_gather_matches_oracle(W, algo):
+    """bf16 parameters: the B2_BF16 gather path on the gradient tensors autograd produced, every explicit algorithm."""
+    d0 = _check_ddp_against_twins(W, lambda: _ragged_mlp(0).to(torch.bfloat16), oracle.B2O_BF16, algo=algo,
+                                  bucket_cap_mb=0.01, first_bucket_mb=0.001)
+    assert len(d0.buckets) >= 2 and d0.gathered_buckets > 0 and d0.copied_in_buckets == 0
+
+
+def test_bucket_of_more_than_max_segments_falls_back_to_copy_in():
+    """65 Linear(8, 8) = 130 parameters in ONE bucket: more than a segment table holds, so the bucket is copied in and
+    reduced in place - still bit for bit the oracle."""
+
+    def deep():
+        torch.manual_seed(0)
+        return nn.Sequential(nn.Linear(64, 8), *[nn.Linear(8, 8) for _ in range(64)]).cuda()
+
+    d0 = _check_ddp_against_twins(2, deep, oracle.B2O_F32_WIRE_BF16)
+    assert len(d0.buckets) == 1 and len(d0.buckets[0].params) == 130 > 128
+    assert d0.copied_in_buckets > 0 and d0.gathered_buckets == 0
+
+
 def test_state_dict_is_module_prefixed_like_torch_ddp_and_backward_failure_recovers():
     from torchx_b200.ddp import Communicator, DistributedDataParallel
 
