@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define B2_ABI_VERSION 2
+#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16 */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -61,6 +61,15 @@ extern "C" {
                               (== torch bf16_compress_hook semantics)                                   */
 #define B2_F32 1           /* fp32 bucket, fp32 on the wire (== DDP default: pre-divide then SUM)         */
 #define B2_BF16 2          /* bf16 bucket, bf16 on the wire, fp32 accumulate, one final rounding          */
+#define B2_F32_WIRE_F16 3  /* fp32 bucket, fp16 on the wire, fp32 result holding fp16-representable values
+                              (== torch fp16_compress_hook semantics):
+                              c_r = f16(float(f16(x)) * scale),  out = float(f16(s))                      */
+#define B2_F16 4           /* fp16 bucket, fp16 on the wire, fp32 accumulate, one final rounding
+                              (== allreduce_hook / the hook-less Reducer on an fp16 bucket):
+                              c_r = f16(float(x) * scale),  out = f16(s)                                  */
+/* fp16 roundings are IEEE binary16 round-to-nearest-even: subnormals are kept, overflow goes to +-inf (never saturates:
+ * GradScaler relies on an overflowed gradient arriving as inf on every rank), a NaN stays a NaN.  Mode numbers 5..7 are
+ * unused and rejected. */
 
 /* ---- algorithm selection --------------------------------------------------------- */
 #define B2_ALGO_AUTO 0
@@ -170,7 +179,7 @@ int b2_comm_trace(b2_comm_t* comm, int enable, uint64_t* out, int max_ctas);
  * In-place averaged/scaled SUM allreduce of `n_elems` elements at device pointer `buf`
  * (any device allocation of this rank; it does not need to be symmetric memory):
  *      buf[i] <- round( sum_{r=0..W-1} wire( scale * buf_r[i] ) )
- * `mode` is one of B2_F32_WIRE_BF16 / B2_F32 / B2_BF16, `algo` one of B2_ALGO_*.
+ * `mode` is one of B2_F32_WIRE_BF16 / B2_F32 / B2_BF16 / B2_F32_WIRE_F16 / B2_F16, `algo` one of B2_ALGO_*.
  * scale is normally 1/W (DDP gradient averaging).  n_elems == 0 is a no-op.
  */
 int b2_allreduce(b2_comm_t* comm, void* buf, size_t n_elems, int mode, float scale, int algo,

@@ -15,7 +15,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "torchx_b200", "lib", "libb200ddp.so")
 
 INTERESTING = ("LDGMC", "MULTIMEM", "RED", "UBLKCP", "SYNCS", "MEMBAR", "CCTL", "F2FP", "STL", "LDL", "BAR", "ERRBAR", "HMMA", "UTC", "FENCE", "ATOM")
-MODES = {0: "f32 bucket, bf16 wire", 1: "bf16 bucket", 2: "f32 bucket, f32 wire"}
+MODES = {0: "f32 bucket, bf16 wire", 1: "f32 bucket, f32 wire", 2: "bf16 bucket", 3: "f32 bucket, fp16 wire", 4: "fp16 bucket"}
 
 
 def demangle(names):

@@ -429,7 +429,7 @@ cudaError_t launch_local(const Src& src, void* buf, unsigned long long n, float 
   // disables it.
   static const bool use_tma = env_size("B2_LOCAL_TMA", 1) != 0;
   static const unsigned long long tma_min = env_size("B2_LOCAL_TMA_MIN_MB", 256) << 20;
-  const unsigned long long nbytes = n * (MODE == B2_BF16 ? 2 : 4);
+  const unsigned long long nbytes = n * ModeTraits<MODE>::kElemBytes;
   int devno = 0;
   cudaGetDevice(&devno);
   const unsigned long long sms = static_cast<unsigned long long>(sm_count(devno));
@@ -461,8 +461,14 @@ cudaError_t launch_mode(const CommDev& d, const Src& src, int mode, int kind, in
       return launch_by_world<B2_F32_WIRE_BF16>(d, src, kind, grid, p, buf, n, scale, s);
     case B2_F32:
       return launch_by_world<B2_F32>(d, src, kind, grid, p, buf, n, scale, s);
-    default:
+    case B2_BF16:
       return launch_by_world<B2_BF16>(d, src, kind, grid, p, buf, n, scale, s);
+    case B2_F32_WIRE_F16:
+      return launch_by_world<B2_F32_WIRE_F16>(d, src, kind, grid, p, buf, n, scale, s);
+    case B2_F16:
+      return launch_by_world<B2_F16>(d, src, kind, grid, p, buf, n, scale, s);
+    default:  // callers validate with known_mode(); never guess a mode
+      return cudaErrorInvalidValue;
   }
 }
 
@@ -484,6 +490,12 @@ int local_pass_impl(const Src& src, void* buf, size_t n_elems, int mode, float s
     case B2_BF16:
       e = launch_local<B2_BF16>(src, buf, n_elems, scale, s);
       break;
+    case B2_F32_WIRE_F16:
+      e = launch_local<B2_F32_WIRE_F16>(src, buf, n_elems, scale, s);
+      break;
+    case B2_F16:
+      e = launch_local<B2_F16>(src, buf, n_elems, scale, s);
+      break;
     default:
       return fail(B2_EINVAL, "unknown mode %d", mode);
   }
@@ -491,8 +503,45 @@ int local_pass_impl(const Src& src, void* buf, size_t n_elems, int mode, float s
   return B2_OK;
 }
 
-size_t elem_bytes(int mode) { return mode == B2_BF16 ? 2 : 4; }
-size_t wire_vec_bytes(int mode) { return mode == B2_F32 ? 32 : 16; }
+// The B2_* modes of include/b200ddp.h; everything below may assume a known mode once this has said yes.
+bool known_mode(int mode) {
+  switch (mode) {
+    case B2_F32_WIRE_BF16:
+    case B2_F32:
+    case B2_BF16:
+    case B2_F32_WIRE_F16:
+    case B2_F16:
+      return true;
+    default:
+      return false;
+  }
+}
+
+template <int MODE>
+constexpr size_t wire_vec_bytes_of() {
+  return kF32Wire<MODE> ? 32 : 16;
+}
+
+size_t elem_bytes(int mode) {
+  switch (mode) {
+    case B2_F32_WIRE_BF16: return ModeTraits<B2_F32_WIRE_BF16>::kElemBytes;
+    case B2_F32: return ModeTraits<B2_F32>::kElemBytes;
+    case B2_BF16: return ModeTraits<B2_BF16>::kElemBytes;
+    case B2_F32_WIRE_F16: return ModeTraits<B2_F32_WIRE_F16>::kElemBytes;
+    case B2_F16: return ModeTraits<B2_F16>::kElemBytes;
+    default: return 0;
+  }
+}
+size_t wire_vec_bytes(int mode) {
+  switch (mode) {
+    case B2_F32_WIRE_BF16: return wire_vec_bytes_of<B2_F32_WIRE_BF16>();
+    case B2_F32: return wire_vec_bytes_of<B2_F32>();
+    case B2_BF16: return wire_vec_bytes_of<B2_BF16>();
+    case B2_F32_WIRE_F16: return wire_vec_bytes_of<B2_F32_WIRE_F16>();
+    case B2_F16: return wire_vec_bytes_of<B2_F16>();
+    default: return 0;
+  }
+}
 
 unsigned next_creation_index(const char* shm_name, uint64_t epoch) {
   static std::mutex mu;
@@ -991,7 +1040,7 @@ uint64_t b2_comm_launch_count(const b2_comm_t* c) { return c ? c->launches : 0; 
 int b2_comm_last_algo(const b2_comm_t* c) { return c ? c->last_algo : B2_EINVAL; }
 
 int b2_auto_algo(int world, int mode, size_t n_elems, int has_multicast) {
-  if (world < 1 || world > B2_MAX_WORLD || (mode != B2_F32_WIRE_BF16 && mode != B2_F32 && mode != B2_BF16))
+  if (world < 1 || world > B2_MAX_WORLD || !known_mode(mode))
     return fail(B2_EINVAL, "b2_auto_algo: bad arguments (world=%d mode=%d)", world, mode);
   if (world == 1 || n_elems == 0) return B2_ALGO_AUTO;  // no collective: the local pass
   const size_t wire = (n_elems + 7) / 8 * wire_vec_bytes(mode);
@@ -1017,8 +1066,7 @@ int b2_local_pass(void* buf, size_t n_elems, int mode, float scale, int device, 
 
 static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int mode, float scale, int algo, void* stream) {
   if (!c) return fail(B2_EINVAL, "null communicator");
-  if (mode != B2_F32_WIRE_BF16 && mode != B2_F32 && mode != B2_BF16)
-    return fail(B2_EINVAL, "unknown mode %d", mode);
+  if (!known_mode(mode)) return fail(B2_EINVAL, "unknown mode %d", mode);
   if (algo != B2_ALGO_AUTO && algo != B2_ALGO_ONESHOT && algo != B2_ALGO_TWOSHOT && algo != B2_ALGO_TWOSHOT_PIPE &&
       algo != B2_ALGO_NVLS && algo != B2_ALGO_TWOSHOT_LL)
     return fail(B2_EINVAL, "unknown algo %d", algo);

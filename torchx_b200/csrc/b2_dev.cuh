@@ -27,9 +27,61 @@ constexpr size_t kDefaultStageBytes = 512ull << 20;  // x2 stages = 1 GiB of the
 // stall of a healthy peer (rank-0 checkpoint / eval, a dataloader hiccup): NCCL's default for the same situation is 600 s.
 constexpr unsigned long long kDefaultTimeoutNs = 600ull * 1000ull * 1000ull * 1000ull;
 
-// "Not written yet" marker of the NVLS output buffers: a 32-bit word that reduced data never contains (as two bf16 lanes or
-// as one fp32 it is a NaN with an all-ones payload; the producer canonicalises such a word to the default NaN first).
+// "Not written yet" marker of the NVLS output buffers: a 32-bit word that reduced data never contains (as two bf16 lanes,
+// as two fp16 lanes or as one fp32 it is a NaN with an all-ones payload; the producer canonicalises such a word to the
+// default NaN first).
 constexpr uint32_t kSentinel = 0xFFFFFFFFu;
+
+// ---- per-mode facts --------------------------------------------------------------------------------
+// Every "which mode" question the kernels and the launch code ask is answered here, so a mode that is not listed fails to
+// compile instead of silently taking another mode's branch.
+enum class WireFmt { kF32, kBF16, kF16 };
+
+template <int MODE>
+struct ModeTraits {
+  static_assert(MODE < 0 && MODE >= 0, "unknown B2 mode: add its ModeTraits specialisation");
+};
+// Elem: the bucket's element type as the kernels access it (16-bit formats as raw bits); kWire: what travels between
+// ranks; kCastIn: the fp32 bucket is rounded to the wire format BEFORE the scale (the hook's `.to(dtype).div_(W)`).
+template <>
+struct ModeTraits<B2_F32_WIRE_BF16> {
+  using Elem = float;
+  static constexpr int kElemBytes = 4;
+  static constexpr WireFmt kWire = WireFmt::kBF16;
+  static constexpr bool kCastIn = true;
+};
+template <>
+struct ModeTraits<B2_F32> {
+  using Elem = float;
+  static constexpr int kElemBytes = 4;
+  static constexpr WireFmt kWire = WireFmt::kF32;
+  static constexpr bool kCastIn = false;
+};
+template <>
+struct ModeTraits<B2_BF16> {
+  using Elem = uint16_t;
+  static constexpr int kElemBytes = 2;
+  static constexpr WireFmt kWire = WireFmt::kBF16;
+  static constexpr bool kCastIn = false;
+};
+template <>
+struct ModeTraits<B2_F32_WIRE_F16> {
+  using Elem = float;
+  static constexpr int kElemBytes = 4;
+  static constexpr WireFmt kWire = WireFmt::kF16;
+  static constexpr bool kCastIn = true;
+};
+template <>
+struct ModeTraits<B2_F16> {
+  using Elem = uint16_t;
+  static constexpr int kElemBytes = 2;
+  static constexpr WireFmt kWire = WireFmt::kF16;
+  static constexpr bool kCastIn = false;
+};
+template <int MODE>
+constexpr bool kF32Wire = ModeTraits<MODE>::kWire == WireFmt::kF32;  // 32-byte wire vecs (else 16 bytes: 8 x 16 bit)
+template <int MODE>
+constexpr bool k16BitBucket = ModeTraits<MODE>::kElemBytes == 2;     // the bucket holds wire-format elements
 
 static_assert(kMaxCtas * kFlagSlotBytes <= (int)kXbarFlagBytes, "xbar flag region too small");
 static_assert((size_t)kMaxCtas * kPipeKinds * kMaxChunks * kFlagSlotBytes <= kPipeFlagBytes, "pipeline flag region too small");
@@ -165,6 +217,15 @@ __device__ __forceinline__ uint4 mm_ld_reduce_bf16x2(const void* p) {
                : "memory");
   return r;
 }
+// The same with f16x2 lanes (SASS LDGMC.E.F32ADD.F16x8.RN): fp32 accumulation inside the switch, one rounding to fp16.
+__device__ __forceinline__ uint4 mm_ld_reduce_f16x2(const void* p) {
+  uint4 r;
+  asm volatile("multimem.ld_reduce.relaxed.sys.global.add.acc::f32.v4.f16x2 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+               : "l"(p)
+               : "memory");
+  return r;
+}
 __device__ __forceinline__ uint4 mm_ld_reduce_f32(const void* p) {
   uint4 r;
   asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4];"
@@ -191,7 +252,8 @@ __device__ __forceinline__ uint4 ld_volatile_u4(const void* p) {
 __device__ __forceinline__ bool has_sentinel(const uint4& q) {
   return q.x == kSentinel || q.y == kSentinel || q.z == kSentinel || q.w == kSentinel;
 }
-// reduced data never carries the sentinel: an all-ones NaN word becomes the default NaN (bf16x2: both lanes)
+// reduced data never carries the sentinel: an all-ones NaN word becomes the default NaN (bf16x2 / f16x2: both lanes;
+// 0x7FFF is a quiet NaN in both 16-bit formats)
 template <bool F32>
 __device__ __forceinline__ uint4 no_sentinel(uint4 q) {
   constexpr uint32_t kNan = F32 ? 0x7FFFFFFFu : 0x7FFF7FFFu;
@@ -212,23 +274,58 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 __device__ __forceinline__ float bf16_lo(uint32_t p) { return __uint_as_float(p << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t p) { return __uint_as_float(p & 0xffff0000u); }
 
-// ---- per-mode traits ---------------------------------------------------------------------------
-// A "vec" is 8 consecutive elements everywhere in this library.
+// fp32 pair -> packed f16x2, IEEE round-to-nearest-even (F2FP.F16.F32.PACK_AB).  Subnormals are kept, overflow gives
+// +-inf (no .satfinite: an overflowed scaled gradient must stay inf), NaN gives a NaN.  Lane order as pack_bf16x2.
+__device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// fp16 -> fp32 is exact (every fp16 value, subnormals included, is an fp32 normal).
+__device__ __forceinline__ float f16_to_f32(uint16_t h) {
+  float f;
+  asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
+  return f;
+}
+__device__ __forceinline__ float f16_lo(uint32_t p) { return f16_to_f32(static_cast<uint16_t>(p & 0xffffu)); }
+__device__ __forceinline__ float f16_hi(uint32_t p) { return f16_to_f32(static_cast<uint16_t>(p >> 16)); }
+
+// The 16-bit wire formats, selected by mode: pack two fp32 into one word (the rounding), widen either lane (exact).
 template <int MODE>
+__device__ __forceinline__ uint32_t pack16(float lo, float hi) {
+  static_assert(!kF32Wire<MODE>, "pack16: 16-bit wire modes only");
+  if constexpr (ModeTraits<MODE>::kWire == WireFmt::kF16) return pack_f16x2(lo, hi);
+  else return pack_bf16x2(lo, hi);
+}
+template <int MODE>
+__device__ __forceinline__ float lo16(uint32_t p) {
+  if constexpr (ModeTraits<MODE>::kWire == WireFmt::kF16) return f16_lo(p);
+  else return bf16_lo(p);
+}
+template <int MODE>
+__device__ __forceinline__ float hi16(uint32_t p) {
+  if constexpr (ModeTraits<MODE>::kWire == WireFmt::kF16) return f16_hi(p);
+  else return bf16_hi(p);
+}
+// One bucket element (as ModeTraits<MODE>::Elem) -> fp32.
+template <int MODE>
+__device__ __forceinline__ float elem_to_f32(typename ModeTraits<MODE>::Elem x) {
+  if constexpr (k16BitBucket<MODE>) return lo16<MODE>(static_cast<uint32_t>(x));
+  else return x;
+}
+
+// ---- wire vecs -----------------------------------------------------------------------------------
+// A "vec" is 8 consecutive elements everywhere in this library.
+template <int MODE, bool F32 = kF32Wire<MODE>>
 struct Wire;  // wire representation of one vec
 
-template <>
-struct Wire<B2_F32_WIRE_BF16> {
+template <int MODE>
+struct Wire<MODE, false> {  // 8 x 16 bit: bf16x2 or f16x2 words
   static constexpr int kBytes = 16;
   uint4 q;
 };
-template <>
-struct Wire<B2_BF16> {
-  static constexpr int kBytes = 16;
-  uint4 q;
-};
-template <>
-struct Wire<B2_F32> {
+template <int MODE>
+struct Wire<MODE, true> {  // 8 x fp32
   static constexpr int kBytes = 32;
   F8 f;
 };
@@ -236,7 +333,7 @@ struct Wire<B2_F32> {
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> ld_wire(const uint8_t* p) {
   Wire<MODE> w;
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     w.f = ldg_f8(reinterpret_cast<const float*>(p));
   } else {
     w.q = ldg_u4(p);
@@ -245,7 +342,7 @@ __device__ __forceinline__ Wire<MODE> ld_wire(const uint8_t* p) {
 }
 template <int MODE>
 __device__ __forceinline__ void st_wire(uint8_t* p, const Wire<MODE>& w) {
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     stg_f8(reinterpret_cast<float*>(p), w.f);
   } else {
     stg_u4(p, w.q);
@@ -256,7 +353,7 @@ __device__ __forceinline__ void st_wire(uint8_t* p, const Wire<MODE>& w) {
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> mm_ld_reduce_wire(const uint8_t* p) {
   Wire<MODE> w;
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     const uint4 a = mm_ld_reduce_f32(p), b = mm_ld_reduce_f32(p + 16);
     w.f.v[0] = __uint_as_float(a.x);
     w.f.v[1] = __uint_as_float(a.y);
@@ -266,6 +363,8 @@ __device__ __forceinline__ Wire<MODE> mm_ld_reduce_wire(const uint8_t* p) {
     w.f.v[5] = __uint_as_float(b.y);
     w.f.v[6] = __uint_as_float(b.z);
     w.f.v[7] = __uint_as_float(b.w);
+  } else if constexpr (ModeTraits<MODE>::kWire == WireFmt::kF16) {
+    w.q = mm_ld_reduce_f16x2(p);
   } else {
     w.q = mm_ld_reduce_bf16x2(p);
   }
@@ -273,7 +372,7 @@ __device__ __forceinline__ Wire<MODE> mm_ld_reduce_wire(const uint8_t* p) {
 }
 template <int MODE>
 __device__ __forceinline__ void mm_st_wire(uint8_t* p, const Wire<MODE>& w) {
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     mm_st_u4(p, make_uint4(__float_as_uint(w.f.v[0]), __float_as_uint(w.f.v[1]), __float_as_uint(w.f.v[2]),
                            __float_as_uint(w.f.v[3])));
     mm_st_u4(p + 16, make_uint4(__float_as_uint(w.f.v[4]), __float_as_uint(w.f.v[5]), __float_as_uint(w.f.v[6]),
@@ -286,7 +385,7 @@ __device__ __forceinline__ void mm_st_wire(uint8_t* p, const Wire<MODE>& w) {
 // ---- sentinel protocol of the NVLS output buffer (see CommDev::nvls_out_off) -----------------------------------------
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> wire_no_sentinel(Wire<MODE> w) {
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     uint4 a = make_uint4(__float_as_uint(w.f.v[0]), __float_as_uint(w.f.v[1]), __float_as_uint(w.f.v[2]), __float_as_uint(w.f.v[3]));
     uint4 b = make_uint4(__float_as_uint(w.f.v[4]), __float_as_uint(w.f.v[5]), __float_as_uint(w.f.v[6]), __float_as_uint(w.f.v[7]));
     a = no_sentinel<true>(a);
@@ -309,7 +408,7 @@ __device__ __forceinline__ Wire<MODE> wire_no_sentinel(Wire<MODE> w) {
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> wire_poll(const uint8_t* p, bool* pending) {
   Wire<MODE> w;
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     const uint4 a = ld_volatile_u4(p), b = ld_volatile_u4(p + 16);
     *pending = has_sentinel(a) || has_sentinel(b);
     w.f.v[0] = __uint_as_float(a.x);
@@ -330,7 +429,7 @@ template <int MODE>
 __device__ __forceinline__ void wire_reset(uint8_t* p) {
   const uint4 s4 = make_uint4(kSentinel, kSentinel, kSentinel, kSentinel);
   stg_u4(p, s4);
-  if constexpr (MODE == B2_F32) stg_u4(p + 16, s4);
+  if constexpr (kF32Wire<MODE>) stg_u4(p + 16, s4);
 }
 
 // wire(scale * x): the value a rank contributes.  Rounding points are part of the contract
@@ -338,10 +437,12 @@ __device__ __forceinline__ void wire_reset(uint8_t* p) {
 //   F32_WIRE_BF16 : bf16( float(bf16(x)) * scale )      == `buf.to(bf16).div_(W)` for W = 2^k
 //   BF16          : bf16( float(x) * scale )            (x is already bf16)
 //   F32           : x * scale                           == Reducer's `mul_out(bucket, grad, 1/W)`
+//   F32_WIRE_F16  : f16( float(f16(x)) * scale )        == `buf.to(fp16).div_(W)` (fp16_compress_hook)
+//   F16           : f16( float(x) * scale )             (x is already fp16)
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> compress(const F8& x, float scale) {
   Wire<MODE> w;
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) w.f.v[i] = __fmul_rn(x.v[i], scale);
   } else {
@@ -349,12 +450,12 @@ __device__ __forceinline__ Wire<MODE> compress(const F8& x, float scale) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float a = x.v[2 * i], b = x.v[2 * i + 1];
-      if constexpr (MODE == B2_F32_WIRE_BF16) {
-        const uint32_t p = pack_bf16x2(a, b);  // first rounding: the `.to(bf16)` cast
-        a = bf16_lo(p);
-        b = bf16_hi(p);
+      if constexpr (ModeTraits<MODE>::kCastIn) {
+        const uint32_t p = pack16<MODE>(a, b);  // first rounding: the `.to(bf16 / fp16)` cast
+        a = lo16<MODE>(p);
+        b = hi16<MODE>(p);
       }
-      o[i] = pack_bf16x2(__fmul_rn(a, scale), __fmul_rn(b, scale));
+      o[i] = pack16<MODE>(__fmul_rn(a, scale), __fmul_rn(b, scale));
     }
     w.q = make_uint4(o[0], o[1], o[2], o[3]);
   }
@@ -363,18 +464,18 @@ __device__ __forceinline__ Wire<MODE> compress(const F8& x, float scale) {
 
 template <int MODE>
 __device__ __forceinline__ F8 widen(const Wire<MODE>& w) {
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     return w.f;
   } else {
     F8 r;
-    r.v[0] = bf16_lo(w.q.x);
-    r.v[1] = bf16_hi(w.q.x);
-    r.v[2] = bf16_lo(w.q.y);
-    r.v[3] = bf16_hi(w.q.y);
-    r.v[4] = bf16_lo(w.q.z);
-    r.v[5] = bf16_hi(w.q.z);
-    r.v[6] = bf16_lo(w.q.w);
-    r.v[7] = bf16_hi(w.q.w);
+    r.v[0] = lo16<MODE>(w.q.x);
+    r.v[1] = hi16<MODE>(w.q.x);
+    r.v[2] = lo16<MODE>(w.q.y);
+    r.v[3] = hi16<MODE>(w.q.y);
+    r.v[4] = lo16<MODE>(w.q.z);
+    r.v[5] = hi16<MODE>(w.q.z);
+    r.v[6] = lo16<MODE>(w.q.w);
+    r.v[7] = hi16<MODE>(w.q.w);
     return r;
   }
 }
@@ -383,11 +484,11 @@ __device__ __forceinline__ F8 widen(const Wire<MODE>& w) {
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> finalize(const F8& s) {
   Wire<MODE> w;
-  if constexpr (MODE == B2_F32) {
+  if constexpr (kF32Wire<MODE>) {
     w.f = s;
   } else {
-    w.q = make_uint4(pack_bf16x2(s.v[0], s.v[1]), pack_bf16x2(s.v[2], s.v[3]),
-                     pack_bf16x2(s.v[4], s.v[5]), pack_bf16x2(s.v[6], s.v[7]));
+    w.q = make_uint4(pack16<MODE>(s.v[0], s.v[1]), pack16<MODE>(s.v[2], s.v[3]),
+                     pack16<MODE>(s.v[4], s.v[5]), pack16<MODE>(s.v[6], s.v[7]));
   }
   return w;
 }
@@ -402,16 +503,16 @@ template <int MODE>
 __device__ __forceinline__ F8 load_in(const void* buf, unsigned long long e, unsigned long long n,
                                       bool aligned) {
   F8 x;
-  if constexpr (MODE == B2_BF16) {
+  if constexpr (k16BitBucket<MODE>) {  // the bucket holds wire-format elements
     const uint16_t* p = reinterpret_cast<const uint16_t*>(buf) + e;
     if (aligned && e + 8 <= n) {
-      Wire<B2_BF16> w;
+      Wire<MODE> w;
       w.q = ldg_u4(p);
-      x = widen<B2_BF16>(w);
+      x = widen<MODE>(w);
     } else {
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        x.v[i] = (e + i < n) ? __uint_as_float(static_cast<uint32_t>(p[i]) << 16) : 0.f;
+        x.v[i] = (e + i < n) ? elem_to_f32<MODE>(p[i]) : 0.f;
     }
   } else {
     const float* p = reinterpret_cast<const float*>(buf) + e;
@@ -429,7 +530,7 @@ __device__ __forceinline__ F8 load_in(const void* buf, unsigned long long e, uns
 template <int MODE>
 __device__ __forceinline__ void store_out(void* buf, unsigned long long e, unsigned long long n,
                                           bool aligned, const Wire<MODE>& w) {
-  if constexpr (MODE == B2_BF16) {
+  if constexpr (k16BitBucket<MODE>) {  // the wire bits are the bucket's bits
     uint16_t* p = reinterpret_cast<uint16_t*>(buf) + e;
     if (aligned && e + 8 <= n) {
       stg_u4(p, w.q);
@@ -454,7 +555,7 @@ __device__ __forceinline__ void store_out(void* buf, unsigned long long e, unsig
 
 template <int MODE>
 __device__ __forceinline__ bool buf_aligned(const void* buf) {
-  return (reinterpret_cast<uintptr_t>(buf) & (MODE == B2_BF16 ? 15u : 31u)) == 0;
+  return (reinterpret_cast<uintptr_t>(buf) & (8u * ModeTraits<MODE>::kElemBytes - 1u)) == 0;  // one vec: 16 or 32 bytes
 }
 
 // One input vec (elements [e, e + 8) of this launch) from wherever `src` says the input lives.
@@ -469,7 +570,7 @@ template <int MODE>
 __device__ __forceinline__ F8 load_src(const Src& src, SegHint& hint, const void* buf, unsigned long long e,
                                        unsigned long long n, bool aligned) {
   if (src.nseg == 0) return load_in<MODE>(buf, e, n, aligned);
-  using Elem = typename std::conditional<MODE == B2_BF16, uint16_t, float>::type;
+  using Elem = typename ModeTraits<MODE>::Elem;
   const unsigned long long ge = e + src.off;  // bucket coordinates
   int s = hint.s;
   unsigned long long sb = hint.sb, se = hint.se;
@@ -490,11 +591,11 @@ __device__ __forceinline__ F8 load_src(const Src& src, SegHint& hint, const void
   const Elem* base = static_cast<const Elem*>(src.ptr[s]);
   const Elem* p = base + (ge - sb);
   F8 x;
-  if (e + 8 <= n && ge + 8 <= se && (reinterpret_cast<uintptr_t>(p) & (MODE == B2_BF16 ? 15u : 31u)) == 0) {
-    if constexpr (MODE == B2_BF16) {
-      Wire<B2_BF16> w;
+  if (e + 8 <= n && ge + 8 <= se && (reinterpret_cast<uintptr_t>(p) & (8u * sizeof(Elem) - 1u)) == 0) {
+    if constexpr (k16BitBucket<MODE>) {
+      Wire<MODE> w;
       w.q = ldg_u4(p);
-      x = widen<B2_BF16>(w);
+      x = widen<MODE>(w);
     } else {
       x = ldg_f8(p);
     }
@@ -510,10 +611,7 @@ __device__ __forceinline__ F8 load_src(const Src& src, SegHint& hint, const void
           se = src.begin[s + 1];
           base = static_cast<const Elem*>(src.ptr[s]);
         }
-        if constexpr (MODE == B2_BF16)
-          v = __uint_as_float(static_cast<uint32_t>(base[g - sb]) << 16);
-        else
-          v = base[g - sb];
+        v = elem_to_f32<MODE>(base[g - sb]);
       }
       x.v[i] = v;
     }

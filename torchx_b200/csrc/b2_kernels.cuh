@@ -87,28 +87,34 @@ __device__ __forceinline__ void bulk_wait_read() {
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
-// x <- round(wire(scale * x)) on one 16-byte group (4 fp32 or 8 bf16), same arithmetic as compress+finalize.
+// x <- round(wire(scale * x)) on one 16-byte group (4 fp32 or 8 16-bit elements), same arithmetic as compress+finalize.
 template <int MODE>
 __device__ __forceinline__ uint4 round16(uint4 q, float scale) {
   using namespace dev;
-  if constexpr (MODE == B2_BF16) {
+  if constexpr (k16BitBucket<MODE>) {
     uint32_t in[4] = {q.x, q.y, q.z, q.w}, out[4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) out[i] = pack_bf16x2(__fmul_rn(bf16_lo(in[i]), scale), __fmul_rn(bf16_hi(in[i]), scale));
+    for (int i = 0; i < 4; ++i) out[i] = pack16<MODE>(__fmul_rn(lo16<MODE>(in[i]), scale), __fmul_rn(hi16<MODE>(in[i]), scale));
     return make_uint4(out[0], out[1], out[2], out[3]);
   } else {
     float f[4] = {__uint_as_float(q.x), __uint_as_float(q.y), __uint_as_float(q.z), __uint_as_float(q.w)};
     uint32_t o[4];
 #pragma unroll
     for (int i = 0; i < 4; i += 2) {
-      if constexpr (MODE == B2_F32) {
+      if constexpr (kF32Wire<MODE>) {
         o[i] = __float_as_uint(__fmul_rn(f[i], scale));
         o[i + 1] = __float_as_uint(__fmul_rn(f[i + 1], scale));
       } else {
-        const uint32_t p = pack_bf16x2(f[i], f[i + 1]);                                        // .to(bf16)
-        const uint32_t r = pack_bf16x2(__fmul_rn(bf16_lo(p), scale), __fmul_rn(bf16_hi(p), scale));  // .div_(W), bf16
-        o[i] = r << 16;             // widen back to fp32: bf16 bits in the high half
-        o[i + 1] = r & 0xffff0000u;
+        static_assert(ModeTraits<MODE>::kCastIn, "an fp32 bucket on a 16-bit wire is rounded to the wire format first");
+        const uint32_t p = pack16<MODE>(f[i], f[i + 1]);                                            // .to(bf16 / fp16)
+        const uint32_t r = pack16<MODE>(__fmul_rn(lo16<MODE>(p), scale), __fmul_rn(hi16<MODE>(p), scale));  // .div_(W)
+        if constexpr (ModeTraits<MODE>::kWire == WireFmt::kBF16) {
+          o[i] = r << 16;             // widen back to fp32: bf16 bits in the high half
+          o[i + 1] = r & 0xffff0000u;
+        } else {
+          o[i] = __float_as_uint(lo16<MODE>(r));  // widen back to fp32 (exact)
+          o[i + 1] = __float_as_uint(hi16<MODE>(r));
+        }
       }
     }
     return make_uint4(o[0], o[1], o[2], o[3]);
@@ -125,7 +131,7 @@ __global__ void __launch_bounds__(tma::kTmaThreads) k_local_pass_tma(void* buf, 
   extern __shared__ __align__(128) uint8_t ring_raw[];  // kStages * kTileBytes of dynamic shared memory
   uint8_t(*ring)[kTileBytes] = reinterpret_cast<uint8_t(*)[kTileBytes]>(ring_raw);
   __shared__ alignas(8) uint64_t full[kStages];
-  constexpr int kElem = MODE == B2_BF16 ? 2 : 4;
+  constexpr int kElem = ModeTraits<MODE>::kElemBytes;
   const unsigned long long bytes = n * kElem;
   const unsigned long long ntiles = bytes / kTileBytes;  // full tiles go through TMA; the tail is handled below
   uint8_t* base = static_cast<uint8_t*>(buf);

@@ -124,9 +124,9 @@ __global__ void __launch_bounds__(kThreads, 1)
       const bool do3 = v0 >= step + first && v0 - step < Ls;
       if (!do2 && !do3) break;
       if (do2) {  // ---- phase 2: reduce my slice as its contributions arrive, push the result to everyone
-        // G contributions of one vec are polled together (all W for the 16-byte bf16 wire vecs; 4 for the 32-byte fp32 ones,
-        // which would not fit the register file otherwise); accumulation stays in rank order either way.
-        constexpr int G = (MODE == B2_F32 && W > 4) ? 4 : W;
+        // G contributions of one vec are polled together (all W for the 16-byte bf16 / fp16 wire vecs; 4 for the 32-byte fp32
+        // ones, which would not fit the register file otherwise); accumulation stays in rank order either way.
+        constexpr int G = (kF32Wire<MODE> && W > 4) ? 4 : W;
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const unsigned long long v = v0 + u * stride;
@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       if (do3) {  // ---- phase 3: widen every slice of the previous trip as it arrives
         const unsigned long long p0 = v0 - step;
-        constexpr int G = (MODE == B2_F32 && W > 4) ? 4 : W;
+        constexpr int G = (kF32Wire<MODE> && W > 4) ? 4 : W;
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const unsigned long long v = p0 + u * stride;

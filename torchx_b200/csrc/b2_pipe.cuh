@@ -193,7 +193,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       group_wait(c, 2, kBD, t, 0, k, seq);
       if (t == 0 && k == 0) trace_stamp(c, 2);
       if constexpr (ALG == kNvls) {
-        constexpr int UM = MODE == B2_F32 ? 4 : 8;  // 128 B of switch-side reductions in flight per thread
+        constexpr int UM = kF32Wire<MODE> ? 4 : 8;  // 128 B of switch-side reductions in flight per thread
         const uint8_t* const mc_in = c.mc + stage;   // every rank's staged contribution, summed by the switch on load
         uint8_t* const mc_out = c.mc + nvls_out + c.rank * c.slice_cap;  // out[me] on every rank, written by the switch on store
         for (unsigned long long v0 = lo + t; v0 < hi; v0 += static_cast<unsigned long long>(kBD) * UM) {

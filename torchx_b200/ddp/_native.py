@@ -17,7 +17,7 @@ SRC_DIR = os.path.join(_PKG, "csrc")
 SRC_PATH = os.path.join(SRC_DIR, "b200ddp.cu")  # the one translation unit; it includes the other files of csrc/
 INCLUDE_DIR = os.path.join(os.path.dirname(_PKG), "include")
 
-B2_ABI_VERSION = 2
+B2_ABI_VERSION = 3
 B2_MAX_WORLD = 8
 
 B2_OK = 0
@@ -32,6 +32,8 @@ B2_ENOTSUP = -7
 B2_F32_WIRE_BF16 = 0
 B2_F32 = 1
 B2_BF16 = 2
+B2_F32_WIRE_F16 = 3
+B2_F16 = 4
 
 B2_ALGO_AUTO = 0
 B2_ALGO_ONESHOT = 1

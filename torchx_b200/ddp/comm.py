@@ -18,19 +18,25 @@ from . import _native as N
 _MODE_FOR = {
     ("f32", "bf16"): N.B2_F32_WIRE_BF16,
     ("f32", "f32"): N.B2_F32,
+    ("f32", "f16"): N.B2_F32_WIRE_F16,
     ("bf16", "bf16"): N.B2_BF16,
+    ("f16", "f16"): N.B2_F16,
 }
 ALGOS = {"auto": N.B2_ALGO_AUTO, "oneshot": N.B2_ALGO_ONESHOT, "twoshot": N.B2_ALGO_TWOSHOT, "twoshot_pipe": N.B2_ALGO_TWOSHOT_PIPE,
          "nvls": N.B2_ALGO_NVLS, "twoshot_ll": N.B2_ALGO_TWOSHOT_LL}
 
 
 def mode_for(tensor: torch.Tensor, wire: str = "bf16") -> int:
+    """The B2_* mode for a bucket of this dtype: fp32 buckets take the wire format `wire` ("bf16", "f16" or "f32"); a
+    16-bit bucket is its own wire format whatever `wire` says."""
     if tensor.dtype == torch.float32:
         key = ("f32", wire)
     elif tensor.dtype == torch.bfloat16:
         key = ("bf16", "bf16")
+    elif tensor.dtype == torch.float16:
+        key = ("f16", "f16")
     else:
-        raise TypeError(f"unsupported gradient dtype {tensor.dtype}; expected float32 or bfloat16")
+        raise TypeError(f"unsupported gradient dtype {tensor.dtype}; expected float32, bfloat16 or float16")
     if key not in _MODE_FOR:
         raise ValueError(f"unsupported wire format {wire!r} for dtype {tensor.dtype}")
     return _MODE_FOR[key]

@@ -7,6 +7,9 @@ bf16 and widened back to fp32), one launch instead of four and no NCCL on the da
 
     ddp = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local_rank])
     ddp.register_comm_hook(B200HookState(comm), b200_bf16_compress_hook)
+
+``b200_fp16_compress_hook`` is the same for ``default_hooks.fp16_compress_hook`` (fp16 on the wire).  A bf16 or fp16
+bucket (a ``.bfloat16()`` / ``.half()`` model) is reduced in its own format by every hook, as ``allreduce_hook`` would.
 """
 from typing import Optional
 
@@ -43,6 +46,12 @@ def _run(state: B200HookState, bucket, wire: str) -> torch.futures.Future[torch.
 
 def b200_bf16_compress_hook(state: B200HookState, bucket) -> torch.futures.Future[torch.Tensor]:
     return _run(state, bucket, "bf16")
+
+
+def b200_fp16_compress_hook(state: B200HookState, bucket) -> torch.futures.Future[torch.Tensor]:
+    """Drop-in for ``default_hooks.fp16_compress_hook``: the bucket is cast to fp16, divided by W, summed and widened back
+    (values rounded to fp16; an overflow arrives as inf on every rank, which is what GradScaler looks for)."""
+    return _run(state, bucket, "f16")
 
 
 def b200_allreduce_hook(state: B200HookState, bucket) -> torch.futures.Future[torch.Tensor]:
