@@ -4,8 +4,15 @@
 instructions (LDGMC / multimem stores), system-scope release/acquire traffic, TMA bulk copies, local-memory spills.
 
     mkdir -p tool_out && python tools/sass_report.py > tool_out/sass_report.md
+
+``--digest [LIB]`` prints one line per kernel instead, ``<demangled name> <sha256 of its SASS>``, for LIB (default: the
+in-tree library).  Two builds whose digests are equal have identical kernels, so a refactor of the device code can be
+checked against the library built from its parent commit:
+
+    diff <(python tools/sass_report.py --digest parent.so) <(python tools/sass_report.py --digest)
 """
 import collections
+import hashlib
 import os
 import re
 import subprocess
@@ -29,10 +36,30 @@ def demangle(names):
     return dict(zip(names, clean))
 
 
+def digest(lib: str) -> None:
+    sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
+    body = collections.defaultdict(list)
+    cur = None
+    for line in sass.splitlines():
+        m = re.match(r"\s*Function : (\S+)", line)
+        if m:
+            cur = m.group(1)
+        elif cur and line.lstrip().startswith("/*"):  # an instruction or the second half of its encoding
+            body[cur].append(line.strip())
+    names = demangle(sorted(body))
+    # the anonymous namespace's hash (in mangled names) changes with any edit to the translation unit
+    anon = re.compile(r"_GLOBAL__N__[0-9a-f]+_")
+    for name, mangled in sorted((anon.sub("_GLOBAL__N__", names[k]), k) for k in body):
+        print(name, hashlib.sha256(anon.sub("_GLOBAL__N__", "\n".join(body[mangled])).encode()).hexdigest())
+
+
 def main() -> None:
     if "-h" in sys.argv or "--help" in sys.argv:
         print(__doc__)
         return
+    if "--digest" in sys.argv:
+        rest = sys.argv[sys.argv.index("--digest") + 1:]
+        return digest(rest[0] if rest else LIB)
     if not os.path.isfile(LIB):
         raise SystemExit(f"{LIB} is not built: python -c 'import __graft_entry__ as g; g.build()'")
     res = subprocess.run(["cuobjdump", "-res-usage", LIB], capture_output=True, text=True, check=True).stdout

@@ -123,6 +123,16 @@ struct LocalMc {
   int refs = 0;
 };
 
+// What B2_ALGO_AUTO picks (auto_algo), in wire bytes of the message.
+struct AutoPolicy {
+  size_t oneshot_max;  // one-shot up to this many
+  size_t ll_min;       // the barrier-free LL two-shot from this many (above the one-shot range) ...
+  size_t ll_max;       // ... up to (excluding) this many
+  size_t pipe_min;     // the pipelined kernels from this many
+  size_t nvls_min;     // NVLS (when available and the mode allows it) from this many ...
+  int nvls_min_world;  // ... and this world size: NVLS only pays once (1 + 1/W) < 2 (W-1)/W
+};
+
 }  // namespace
 
 struct b2_comm {
@@ -144,12 +154,7 @@ struct b2_comm {
   uint32_t* status_host = nullptr;
   // tuning (identical on every rank: they come from the same environment / the same b2_comm_set_param calls)
   int max_ctas = 0;                 // 0 = heuristic
-  size_t oneshot_max_wire_bytes = 0;  // AUTO: one-shot up to this many wire bytes
-  size_t pipe_min_wire_bytes = 0;     // AUTO: the pipelined kernels from this many wire bytes
-  size_t nvls_min_wire_bytes = 0;     // AUTO: NVLS (when available and the mode allows it) from this many wire bytes
-  int nvls_min_world = 4;             // AUTO: NVLS only pays once (1 + 1/W) < 2 (W-1)/W, i.e. W >= 4
-  size_t ll_min_wire_bytes = 0;       // AUTO: the barrier-free LL two-shot from this many wire bytes (above the one-shot range) ...
-  size_t ll_max_wire_bytes = 0;       // ... up to (excluding) this many
+  AutoPolicy policy{};
   size_t pipe_chunk_bytes = 0;        // target wire bytes of one pipeline chunk (per rank)
   uint64_t launches = 0;
   int last_algo = 0;                  // B2_ALGO_* of the most recent allreduce launch (what AUTO picked)
@@ -176,12 +181,6 @@ size_t default_oneshot_max(int world) {
   return 512u << 10;
 }
 
-// What B2_ALGO_AUTO resolves to for one launch (DESIGN.md 2.6).  Pure: the same inputs give the same answer on every rank.
-struct AutoPolicy {
-  size_t oneshot_max, ll_min, ll_max, pipe_min, nvls_min;
-  int nvls_min_world;
-};
-
 AutoPolicy default_policy(int world) {
   AutoPolicy p;
   p.oneshot_max = env_size("B2_ONESHOT_MAX_BYTES", default_oneshot_max(world));
@@ -193,6 +192,7 @@ AutoPolicy default_policy(int world) {
   return p;
 }
 
+// What B2_ALGO_AUTO resolves to for one launch (DESIGN.md 2.6).  Pure: the same inputs give the same answer on every rank.
 int auto_algo(const AutoPolicy& p, int world, int mode, size_t wire_bytes, bool multicast, bool fits_oneshot) {
   // fp32-wire NVLS would let the switch pick the fp32 summation order; AUTO keeps that mode on the rank-order kernels
   if (multicast && mode != B2_F32 && world >= p.nvls_min_world && wire_bytes >= p.nvls_min) return B2_ALGO_NVLS;
@@ -240,13 +240,7 @@ int init_rank(b2_comm* c, int rank, int world, int device, size_t stage_bytes) {
   //   NVLS                from 64 MiB at W = 8; the switch's arithmetic, within one bf16 ulp of the exact sum (DESIGN.md 2.4)
   //   pipelined two-shot  never (explicit choice only)
   // The crossovers have not been re-measured on multi-GPU H100 systems.
-  const AutoPolicy pol = default_policy(world);
-  c->oneshot_max_wire_bytes = pol.oneshot_max;
-  c->pipe_min_wire_bytes = pol.pipe_min;
-  c->nvls_min_wire_bytes = pol.nvls_min;
-  c->nvls_min_world = pol.nvls_min_world;
-  c->ll_min_wire_bytes = pol.ll_min;
-  c->ll_max_wire_bytes = pol.ll_max;
+  c->policy = default_policy(world);
   c->pipe_chunk_bytes = env_size("B2_PIPE_CHUNK_KB", 2048) << 10;
   B2_CUDA(cudaSetDevice(device));
   B2_CUDA(cudaMalloc(&c->counters, 256));
@@ -326,8 +320,6 @@ int grid_for(const b2_comm* c, unsigned long long vecs_per_cta_dim, int unroll) 
   return static_cast<int>(g);
 }
 
-int unroll_for_world(int w) { return w >= 5 ? 1 : (w >= 3 ? 2 : (w >= 2 ? 4 : 8)); }
-
 // SMs of `device` (132 on an H100 SXM, 114 on the PCIe card): the occupancy-sized grids of the local pass scale with it.
 int sm_count(int device) {
   int n = 0;
@@ -365,60 +357,33 @@ PipePlan plan_pipe(const b2_comm* c, unsigned long long Ls, size_t wire_bytes) {
   return p;
 }
 
-template <int MODE, int W>
-cudaError_t launch_oneshot(const CommDev& d, const Src& src, int grid, void* buf, unsigned long long n, float scale,
-                           cudaStream_t s) {
-  k_oneshot<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
-  return cudaGetLastError();
-}
-template <int MODE, int W>
-cudaError_t launch_twoshot(const CommDev& d, const Src& src, int grid, void* buf, unsigned long long n, float scale,
-                           cudaStream_t s) {
-  k_twoshot<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
-  return cudaGetLastError();
-}
-template <int MODE, int W>
-cudaError_t launch_ll(const CommDev& d, const Src& src, int grid, void* buf, unsigned long long n, float scale, cudaStream_t s) {
-  k_ll<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
-  return cudaGetLastError();
-}
-template <int MODE, int W, int ALG>
-cudaError_t launch_pipe(const CommDev& d, const Src& src, const PipePlan& p, void* buf, unsigned long long n, float scale,
-                        cudaStream_t s) {
-  k_pipe<MODE, W, ALG><<<p.grid, kThreads, 0, s>>>(d, src, buf, n, scale, p.K, p.cell);
-  return cudaGetLastError();
-}
-
-// kind: one of B2_ALGO_ONESHOT / TWOSHOT / TWOSHOT_PIPE / NVLS
-template <int MODE>
-cudaError_t launch_by_world(const CommDev& d, const Src& src, int kind, int grid, const PipePlan& p, void* buf,
-                            unsigned long long n, float scale, cudaStream_t s) {
-#define B2_CASE(Wv)                                                                                  \
-  case Wv:                                                                                           \
-    switch (kind) {                                                                                  \
-      case B2_ALGO_ONESHOT:                                                                          \
-        return launch_oneshot<MODE, Wv>(d, src, grid, buf, n, scale, s);                                  \
-      case B2_ALGO_TWOSHOT:                                                                          \
-        return launch_twoshot<MODE, Wv>(d, src, grid, buf, n, scale, s);                                  \
-      case B2_ALGO_TWOSHOT_PIPE:                                                                     \
-        return launch_pipe<MODE, Wv, pl::kP2p>(d, src, p, buf, n, scale, s);                            \
-      case B2_ALGO_TWOSHOT_LL:                                                                       \
-        return launch_ll<MODE, Wv>(d, src, grid, buf, n, scale, s);                                  \
-      default:                                                                                       \
-        return launch_pipe<MODE, Wv, pl::kNvls>(d, src, p, buf, n, scale, s);                           \
+// One collective of `kind` (B2_ALGO_ONESHOT / TWOSHOT / TWOSHOT_PIPE / TWOSHOT_LL / NVLS) at the communicator's world
+// size: instantiates the collective kernels of MODE for W = 2 .. B2_MAX_WORLD.
+template <int MODE, int W = 2>
+cudaError_t launch_collective(const CommDev& d, const Src& src, int kind, int grid, const PipePlan& p, void* buf,
+                              unsigned long long n, float scale, cudaStream_t s) {
+  if constexpr (W > B2_MAX_WORLD) {
+    return cudaErrorInvalidValue;
+  } else {
+    if (d.world != W) return launch_collective<MODE, W + 1>(d, src, kind, grid, p, buf, n, scale, s);
+    switch (kind) {
+      case B2_ALGO_ONESHOT:
+        k_oneshot<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
+        break;
+      case B2_ALGO_TWOSHOT:
+        k_twoshot<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
+        break;
+      case B2_ALGO_TWOSHOT_PIPE:
+        k_pipe<MODE, W, pl::kP2p><<<p.grid, kThreads, 0, s>>>(d, src, buf, n, scale, p.K, p.cell);
+        break;
+      case B2_ALGO_TWOSHOT_LL:
+        k_ll<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
+        break;
+      default:  // B2_ALGO_NVLS
+        k_pipe<MODE, W, pl::kNvls><<<p.grid, kThreads, 0, s>>>(d, src, buf, n, scale, p.K, p.cell);
     }
-  switch (d.world) {
-    B2_CASE(2)
-    B2_CASE(3)
-    B2_CASE(4)
-    B2_CASE(5)
-    B2_CASE(6)
-    B2_CASE(7)
-    B2_CASE(8)
-    default:
-      return cudaErrorInvalidValue;
+    return cudaGetLastError();
   }
-#undef B2_CASE
 }
 
 template <int MODE>
@@ -454,22 +419,45 @@ cudaError_t launch_local(const Src& src, void* buf, unsigned long long n, float 
   return cudaGetLastError();
 }
 
-cudaError_t launch_mode(const CommDev& d, const Src& src, int mode, int kind, int grid, const PipePlan& p, void* buf,
-                        unsigned long long n, float scale, cudaStream_t s) {
+// The B2_* modes of include/b200ddp.h: calls f(std::integral_constant<int, MODE>{}) and returns true, or returns false
+// for an unknown mode.  Every runtime mode becomes a compile-time one here, so a new mode is one more case.
+template <class F>
+bool with_mode(int mode, F&& f) {
   switch (mode) {
     case B2_F32_WIRE_BF16:
-      return launch_by_world<B2_F32_WIRE_BF16>(d, src, kind, grid, p, buf, n, scale, s);
+      f(std::integral_constant<int, B2_F32_WIRE_BF16>{});
+      return true;
     case B2_F32:
-      return launch_by_world<B2_F32>(d, src, kind, grid, p, buf, n, scale, s);
+      f(std::integral_constant<int, B2_F32>{});
+      return true;
     case B2_BF16:
-      return launch_by_world<B2_BF16>(d, src, kind, grid, p, buf, n, scale, s);
+      f(std::integral_constant<int, B2_BF16>{});
+      return true;
     case B2_F32_WIRE_F16:
-      return launch_by_world<B2_F32_WIRE_F16>(d, src, kind, grid, p, buf, n, scale, s);
+      f(std::integral_constant<int, B2_F32_WIRE_F16>{});
+      return true;
     case B2_F16:
-      return launch_by_world<B2_F16>(d, src, kind, grid, p, buf, n, scale, s);
-    default:  // callers validate with known_mode(); never guess a mode
-      return cudaErrorInvalidValue;
+      f(std::integral_constant<int, B2_F16>{});
+      return true;
+    default:
+      return false;
   }
+}
+
+bool known_mode(int mode) {
+  return with_mode(mode, [](auto) {});
+}
+
+size_t elem_bytes(int mode) {
+  size_t b = 0;
+  with_mode(mode, [&](auto m) { b = ModeTraits<decltype(m)::value>::kElemBytes; });
+  return b;
+}
+
+size_t wire_vec_bytes(int mode) {
+  size_t b = 0;
+  with_mode(mode, [&](auto m) { b = dev::Wire<decltype(m)::value>::kBytes; });
+  return b;
 }
 
 const Src kNoSrc = {};  // nseg == 0: the collective reads the bucket itself
@@ -479,68 +467,11 @@ int local_pass_impl(const Src& src, void* buf, size_t n_elems, int mode, float s
   if (!buf) return fail(B2_EINVAL, "b2_local_pass: null buffer");
   DeviceGuard g(device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e;
-  switch (mode) {
-    case B2_F32_WIRE_BF16:
-      e = launch_local<B2_F32_WIRE_BF16>(src, buf, n_elems, scale, s);
-      break;
-    case B2_F32:
-      e = launch_local<B2_F32>(src, buf, n_elems, scale, s);
-      break;
-    case B2_BF16:
-      e = launch_local<B2_BF16>(src, buf, n_elems, scale, s);
-      break;
-    case B2_F32_WIRE_F16:
-      e = launch_local<B2_F32_WIRE_F16>(src, buf, n_elems, scale, s);
-      break;
-    case B2_F16:
-      e = launch_local<B2_F16>(src, buf, n_elems, scale, s);
-      break;
-    default:
-      return fail(B2_EINVAL, "unknown mode %d", mode);
-  }
+  cudaError_t e = cudaSuccess;
+  if (!with_mode(mode, [&](auto m) { e = launch_local<decltype(m)::value>(src, buf, n_elems, scale, s); }))
+    return fail(B2_EINVAL, "unknown mode %d", mode);
   if (e != cudaSuccess) return fail(B2_ECUDA, "k_local_pass launch: %s", cudaGetErrorString(e));
   return B2_OK;
-}
-
-// The B2_* modes of include/b200ddp.h; everything below may assume a known mode once this has said yes.
-bool known_mode(int mode) {
-  switch (mode) {
-    case B2_F32_WIRE_BF16:
-    case B2_F32:
-    case B2_BF16:
-    case B2_F32_WIRE_F16:
-    case B2_F16:
-      return true;
-    default:
-      return false;
-  }
-}
-
-template <int MODE>
-constexpr size_t wire_vec_bytes_of() {
-  return kF32Wire<MODE> ? 32 : 16;
-}
-
-size_t elem_bytes(int mode) {
-  switch (mode) {
-    case B2_F32_WIRE_BF16: return ModeTraits<B2_F32_WIRE_BF16>::kElemBytes;
-    case B2_F32: return ModeTraits<B2_F32>::kElemBytes;
-    case B2_BF16: return ModeTraits<B2_BF16>::kElemBytes;
-    case B2_F32_WIRE_F16: return ModeTraits<B2_F32_WIRE_F16>::kElemBytes;
-    case B2_F16: return ModeTraits<B2_F16>::kElemBytes;
-    default: return 0;
-  }
-}
-size_t wire_vec_bytes(int mode) {
-  switch (mode) {
-    case B2_F32_WIRE_BF16: return wire_vec_bytes_of<B2_F32_WIRE_BF16>();
-    case B2_F32: return wire_vec_bytes_of<B2_F32>();
-    case B2_BF16: return wire_vec_bytes_of<B2_BF16>();
-    case B2_F32_WIRE_F16: return wire_vec_bytes_of<B2_F32_WIRE_F16>();
-    case B2_F16: return wire_vec_bytes_of<B2_F16>();
-    default: return 0;
-  }
 }
 
 unsigned next_creation_index(const char* shm_name, uint64_t epoch) {
@@ -557,6 +488,13 @@ bool wait_count(std::atomic<int>& ctr, int target, std::atomic<int>* abort_flag,
     usleep(200);
   }
   return true;
+}
+
+// A kernel that gave up waiting for a peer leaves the communicator's buffers and counters in an unknown state.
+int check_not_poisoned(const b2_comm* c) {
+  if (*reinterpret_cast<volatile uint32_t*>(c->status_host) != 0)
+    return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
+  return B2_OK;
 }
 
 // Multi-process multicast bring-up (after every rank has mapped every peer arena).  Any failure on any rank sets
@@ -1015,12 +953,12 @@ int b2_comm_set_max_ctas(b2_comm_t* c, int max_ctas) {
 int b2_comm_set_param(b2_comm_t* c, const char* name, long long value) {
   if (!c || !name || value < 0) return fail(B2_EINVAL, "b2_comm_set_param: bad arguments");
   const std::string k(name);
-  if (k == "oneshot_max_bytes") c->oneshot_max_wire_bytes = static_cast<size_t>(value);
-  else if (k == "pipe_min_bytes") c->pipe_min_wire_bytes = static_cast<size_t>(value);
-  else if (k == "nvls_min_bytes") c->nvls_min_wire_bytes = static_cast<size_t>(value);
-  else if (k == "nvls_min_world") c->nvls_min_world = static_cast<int>(value);
-  else if (k == "ll_min_bytes") c->ll_min_wire_bytes = static_cast<size_t>(value);
-  else if (k == "ll_max_bytes") c->ll_max_wire_bytes = static_cast<size_t>(value);
+  if (k == "oneshot_max_bytes") c->policy.oneshot_max = static_cast<size_t>(value);
+  else if (k == "pipe_min_bytes") c->policy.pipe_min = static_cast<size_t>(value);
+  else if (k == "nvls_min_bytes") c->policy.nvls_min = static_cast<size_t>(value);
+  else if (k == "nvls_min_world") c->policy.nvls_min_world = static_cast<int>(value);
+  else if (k == "ll_min_bytes") c->policy.ll_min = static_cast<size_t>(value);
+  else if (k == "ll_max_bytes") c->policy.ll_max = static_cast<size_t>(value);
   else if (k == "pipe_chunk_bytes") c->pipe_chunk_bytes = static_cast<size_t>(value);
   else if (k == "max_ctas") c->max_ctas = static_cast<int>(value);
   else return fail(B2_EINVAL, "b2_comm_set_param: unknown parameter '%s'", name);
@@ -1072,8 +1010,7 @@ static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int
     return fail(B2_EINVAL, "unknown algo %d", algo);
   if (n_elems == 0) return B2_OK;
   if (!buf) return fail(B2_EINVAL, "b2_allreduce: null buffer");
-  if (*reinterpret_cast<volatile uint32_t*>(c->status_host) != 0)
-    return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
+  if (const int rc = check_not_poisoned(c)) return rc;
   const int W = c->d.world;
   if (W == 1) {
     if (mode == B2_F32 && scale == 1.0f && src.nseg == 0) return B2_OK;  // identity
@@ -1087,7 +1024,7 @@ static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t wvb = wire_vec_bytes(mode);
   const size_t cap_vecs = c->d.slice_cap / wvb;  // vecs one region can hold
-  const int U = unroll_for_world(W);
+  const int U = vecs_per_trip(W);
   uint8_t* p = static_cast<uint8_t*>(buf);
   size_t left = n_elems;
   while (left > 0) {
@@ -1095,9 +1032,7 @@ static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int
     const size_t wire_left = V_left * wvb;
     int kind;
     if (algo == B2_ALGO_AUTO) {
-      AutoPolicy pol{c->oneshot_max_wire_bytes, c->ll_min_wire_bytes, c->ll_max_wire_bytes, c->pipe_min_wire_bytes,
-                     c->nvls_min_wire_bytes, c->nvls_min_world};
-      kind = auto_algo(pol, W, mode, wire_left, c->d.mc != nullptr, V_left <= cap_vecs);
+      kind = auto_algo(c->policy, W, mode, wire_left, c->d.mc != nullptr, V_left <= cap_vecs);
     } else {
       kind = algo;
     }
@@ -1108,7 +1043,8 @@ static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int
     const unsigned long long Ls = (V + W - 1) / W;
     const PipePlan plan = plan_pipe(c, Ls, V * wvb);
     const int grid = grid_for(c, oneshot ? V : Ls, U);
-    const cudaError_t e = launch_mode(c->d, src, mode, kind, grid, plan, p, n, scale, s);
+    cudaError_t e = cudaErrorInvalidValue;  // never guess a mode
+    with_mode(mode, [&](auto m) { e = launch_collective<decltype(m)::value>(c->d, src, kind, grid, plan, p, n, scale, s); });
     if (e != cudaSuccess) return fail(B2_ECUDA, "allreduce kernel launch: %s", cudaGetErrorString(e));
     c->launches++;
     c->last_algo = kind;
@@ -1151,8 +1087,7 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
   if (root < 0 || root >= c->d.world) return fail(B2_EINVAL, "b2_broadcast: root %d out of range", root);
   if (bytes == 0 || c->d.world == 1) return B2_OK;
   if (!buf) return fail(B2_EINVAL, "b2_broadcast: null buffer");
-  if (*reinterpret_cast<volatile uint32_t*>(c->status_host) != 0)
-    return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
+  if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t cap = c->stage_bytes & ~static_cast<size_t>(15);
@@ -1174,8 +1109,7 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
 int b2_barrier(b2_comm_t* c, void* stream) {
   if (!c) return fail(B2_EINVAL, "null communicator");
   if (c->d.world == 1) return B2_OK;
-  if (*reinterpret_cast<volatile uint32_t*>(c->status_host) != 0)
-    return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
+  if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
   k_barrier<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(c->d);
   cudaError_t e = cudaGetLastError();

@@ -27,6 +27,10 @@ constexpr size_t kDefaultStageBytes = 512ull << 20;  // x2 stages = 1 GiB of the
 // stall of a healthy peer (rank-0 checkpoint / eval, a dataloader hiccup): NCCL's default for the same situation is 600 s.
 constexpr unsigned long long kDefaultTimeoutNs = 600ull * 1000ull * 1000ull * 1000ull;
 
+// Vecs per thread per loop trip of the multi-rank kernels: U x W wire vecs in flight per thread, without spilling
+// (U*W*8 data registers).  The host sizes their grids with the same number.
+__host__ __device__ constexpr int vecs_per_trip(int world) { return world >= 5 ? 1 : (world >= 3 ? 2 : (world >= 2 ? 4 : 8)); }
+
 // "Not written yet" marker of the NVLS output buffers: a 32-bit word that reduced data never contains (as two bf16 lanes,
 // as two fp16 lanes or as one fp32 it is a NaN with an all-ones payload; the producer canonicalises such a word to the
 // default NaN first).
@@ -147,6 +151,16 @@ namespace dev {
 struct F8 {
   float v[8];
 };
+
+// An 8-float vec as the two 16-byte words it travels in, and back (bit casts, no arithmetic).
+__device__ __forceinline__ void f8_to_u4(const F8& f, uint4& a, uint4& b) {
+  a = make_uint4(__float_as_uint(f.v[0]), __float_as_uint(f.v[1]), __float_as_uint(f.v[2]), __float_as_uint(f.v[3]));
+  b = make_uint4(__float_as_uint(f.v[4]), __float_as_uint(f.v[5]), __float_as_uint(f.v[6]), __float_as_uint(f.v[7]));
+}
+__device__ __forceinline__ F8 f8_from_u4(const uint4& a, const uint4& b) {
+  return F8{{__uint_as_float(a.x), __uint_as_float(a.y), __uint_as_float(a.z), __uint_as_float(a.w),
+             __uint_as_float(b.x), __uint_as_float(b.y), __uint_as_float(b.z), __uint_as_float(b.w)}};
+}
 
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -355,14 +369,7 @@ __device__ __forceinline__ Wire<MODE> mm_ld_reduce_wire(const uint8_t* p) {
   Wire<MODE> w;
   if constexpr (kF32Wire<MODE>) {
     const uint4 a = mm_ld_reduce_f32(p), b = mm_ld_reduce_f32(p + 16);
-    w.f.v[0] = __uint_as_float(a.x);
-    w.f.v[1] = __uint_as_float(a.y);
-    w.f.v[2] = __uint_as_float(a.z);
-    w.f.v[3] = __uint_as_float(a.w);
-    w.f.v[4] = __uint_as_float(b.x);
-    w.f.v[5] = __uint_as_float(b.y);
-    w.f.v[6] = __uint_as_float(b.z);
-    w.f.v[7] = __uint_as_float(b.w);
+    w.f = f8_from_u4(a, b);
   } else if constexpr (ModeTraits<MODE>::kWire == WireFmt::kF16) {
     w.q = mm_ld_reduce_f16x2(p);
   } else {
@@ -373,10 +380,10 @@ __device__ __forceinline__ Wire<MODE> mm_ld_reduce_wire(const uint8_t* p) {
 template <int MODE>
 __device__ __forceinline__ void mm_st_wire(uint8_t* p, const Wire<MODE>& w) {
   if constexpr (kF32Wire<MODE>) {
-    mm_st_u4(p, make_uint4(__float_as_uint(w.f.v[0]), __float_as_uint(w.f.v[1]), __float_as_uint(w.f.v[2]),
-                           __float_as_uint(w.f.v[3])));
-    mm_st_u4(p + 16, make_uint4(__float_as_uint(w.f.v[4]), __float_as_uint(w.f.v[5]), __float_as_uint(w.f.v[6]),
-                                __float_as_uint(w.f.v[7])));
+    uint4 a, b;
+    f8_to_u4(w.f, a, b);
+    mm_st_u4(p, a);
+    mm_st_u4(p + 16, b);
   } else {
     mm_st_u4(p, w.q);
   }
@@ -386,18 +393,9 @@ __device__ __forceinline__ void mm_st_wire(uint8_t* p, const Wire<MODE>& w) {
 template <int MODE>
 __device__ __forceinline__ Wire<MODE> wire_no_sentinel(Wire<MODE> w) {
   if constexpr (kF32Wire<MODE>) {
-    uint4 a = make_uint4(__float_as_uint(w.f.v[0]), __float_as_uint(w.f.v[1]), __float_as_uint(w.f.v[2]), __float_as_uint(w.f.v[3]));
-    uint4 b = make_uint4(__float_as_uint(w.f.v[4]), __float_as_uint(w.f.v[5]), __float_as_uint(w.f.v[6]), __float_as_uint(w.f.v[7]));
-    a = no_sentinel<true>(a);
-    b = no_sentinel<true>(b);
-    w.f.v[0] = __uint_as_float(a.x);
-    w.f.v[1] = __uint_as_float(a.y);
-    w.f.v[2] = __uint_as_float(a.z);
-    w.f.v[3] = __uint_as_float(a.w);
-    w.f.v[4] = __uint_as_float(b.x);
-    w.f.v[5] = __uint_as_float(b.y);
-    w.f.v[6] = __uint_as_float(b.z);
-    w.f.v[7] = __uint_as_float(b.w);
+    uint4 a, b;
+    f8_to_u4(w.f, a, b);
+    w.f = f8_from_u4(no_sentinel<true>(a), no_sentinel<true>(b));
   } else {
     w.q = no_sentinel<false>(w.q);
   }
@@ -411,14 +409,7 @@ __device__ __forceinline__ Wire<MODE> wire_poll(const uint8_t* p, bool* pending)
   if constexpr (kF32Wire<MODE>) {
     const uint4 a = ld_volatile_u4(p), b = ld_volatile_u4(p + 16);
     *pending = has_sentinel(a) || has_sentinel(b);
-    w.f.v[0] = __uint_as_float(a.x);
-    w.f.v[1] = __uint_as_float(a.y);
-    w.f.v[2] = __uint_as_float(a.z);
-    w.f.v[3] = __uint_as_float(a.w);
-    w.f.v[4] = __uint_as_float(b.x);
-    w.f.v[5] = __uint_as_float(b.y);
-    w.f.v[6] = __uint_as_float(b.z);
-    w.f.v[7] = __uint_as_float(b.w);
+    w.f = f8_from_u4(a, b);
   } else {
     w.q = ld_volatile_u4(p);
     *pending = has_sentinel(w.q);
@@ -496,6 +487,16 @@ __device__ __forceinline__ Wire<MODE> finalize(const F8& s) {
 __device__ __forceinline__ void accumulate(F8& s, const F8& c) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) s.v[i] = __fadd_rn(s.v[i], c.v[i]);
+}
+
+// The W contributions to one vec summed in rank order, in fp32 (oracle/allreduce_oracle.c: b2o_allreduce).  k_twoshot and
+// k_pipe take the sum in a statement of its own before the store: as an argument of st_wire it reorders their SASS.
+template <int MODE, int W>
+__device__ __forceinline__ F8 reduce_rank_order(const Wire<MODE> (&w)[W]) {
+  F8 s = widen<MODE>(w[0]);
+#pragma unroll
+  for (int r = 1; r < W; ++r) accumulate(s, widen<MODE>(w[r]));
+  return s;
 }
 
 // ---- local bucket accesses (the caller's tensor: any alignment, any length) --------------------
@@ -635,6 +636,21 @@ __device__ __forceinline__ uint8_t* peer_sel(const CommDev& c, int jj) {
   return a;
 }
 
+// Rank whose slice a rank visits jj-th (jj < 2W): (rank + jj) mod W, the order peer[] is rotated in.
+template <int W>
+__device__ __forceinline__ int slice_of(int rank, int jj) {
+  int j = rank + jj;
+  if (j >= W) j -= W;
+  return j;
+}
+
+// A peer wait gave up: record it in the host-mapped status word (b2_comm_status).  Results are undefined from here on,
+// but the GPU is not hung.
+__device__ __forceinline__ void record_timeout(const CommDev& c) {
+  *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
+  __threadfence_system();
+}
+
 // Bounded wait until *flag >= seq (wrap-safe).  Polls with ld.acquire.sys itself rather than relaxed polling + one
 // fence.acq_rel.sys at the end: the standalone fence is a full MEMBAR.SYS that also drains this SM's outstanding stores,
 // the acquire load is not.
@@ -647,9 +663,31 @@ __device__ __forceinline__ void wait_flag(const CommDev& c, const uint32_t* flag
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > c.timeout_ns) {
-        *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
-        __threadfence_system();
-        break;  // give up: results are undefined, but the GPU is not hung; the host sees the status word
+        record_timeout(c);
+        break;
+      }
+    }
+  }
+}
+
+// Poll one wire vec until no word holds the sentinel, sleeping kSleepNs between polls and reading the clock every
+// kClockEvery (a power of two) polls; bounded like every other wait.
+template <int MODE, unsigned kSleepNs, unsigned kClockEvery>
+__device__ __forceinline__ void wait_wire(const CommDev& c, const uint8_t* p, Wire<MODE>& w) {
+  static_assert((kClockEvery & (kClockEvery - 1u)) == 0, "kClockEvery must be a power of two");
+  unsigned long long t0 = 0;
+  unsigned spins = 0;
+  bool pending = true;
+  while (pending) {
+    __nanosleep(kSleepNs);
+    w = wire_poll<MODE>(p, &pending);
+    if (pending && (++spins & (kClockEvery - 1u)) == 0) {
+      const unsigned long long now = globaltimer_ns();
+      if (t0 == 0) {
+        t0 = now;
+      } else if (now - t0 > c.timeout_ns) {
+        record_timeout(c);
+        break;
       }
     }
   }
@@ -694,10 +732,5 @@ __device__ __forceinline__ void op_end(const CommDev& c, uint32_t seq0) {
 __device__ __forceinline__ void trace_stamp(const CommDev& c, int slot) {
   if (c.trace != nullptr) c.trace[blockIdx.x * 8 + slot] = globaltimer_ns();
 }
-
-template <int W>
-struct Unroll {  // vecs per thread per loop trip: U x W wire vecs in flight per thread, without spilling (U*W*8 data registers)
-  static constexpr int kU = (W >= 5) ? 1 : (W >= 3 ? 2 : (W >= 2 ? 4 : 8));
-};
 
 }  // namespace dev

@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     k_oneshot(CommDev c, const __grid_constant__ Src src, void* buf, unsigned long long n, float scale) {
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
-  constexpr int U = Unroll<W>::kU;
+  constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
   const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
   const bool aligned = buf_aligned<MODE>(buf);
@@ -243,10 +243,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     for (int u = 0; u < U; ++u) {
       const unsigned long long v = v0 + u * stride;
       if (v < V) {
-        F8 s = widen<MODE>(w[u][0]);
-#pragma unroll
-        for (int r = 1; r < W; ++r) accumulate(s, widen<MODE>(w[u][r]));
-        store_out<MODE>(buf, v * 8, n, aligned, finalize<MODE>(s));
+        store_out<MODE>(buf, v * 8, n, aligned, finalize<MODE>(reduce_rank_order<MODE, W>(w[u])));
       }
     }
   }
@@ -268,7 +265,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     k_twoshot(CommDev c, const __grid_constant__ Src src, void* buf, unsigned long long n, float scale) {
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
-  constexpr int U = Unroll<W>::kU;
+  constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
   const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
   const bool aligned = buf_aligned<MODE>(buf);
@@ -288,8 +285,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V) x[u][jj] = load_src<MODE>(src, buf, gv * 8, n, aligned);
       }
@@ -299,8 +295,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V)
           st_wire<MODE>(c.peer[jj] + my_recv + v * WVB, compress<MODE>(x[u][jj], scale));
@@ -330,9 +325,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       for (int u = 0; u < U; ++u) {
         const unsigned long long v = v0 + u * stride;
         if (v < Ls && base + v < V) {
-          F8 s = widen<MODE>(w[u][0]);
-#pragma unroll
-          for (int r = 1; r < W; ++r) accumulate(s, widen<MODE>(w[u][r]));
+          const F8 s = reduce_rank_order<MODE, W>(w[u]);
           st_wire<MODE>(mine + reduced + v * WVB, finalize<MODE>(s));
         }
       }
@@ -350,8 +343,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V) w[u][jj] = ld_wire<MODE>(c.peer[jj] + reduced + v * WVB);
       }
@@ -361,8 +353,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V) store_out<MODE>(buf, gv * 8, n, aligned, w[u][jj]);
       }

@@ -25,37 +25,12 @@
 
 #include "b2_dev.cuh"
 
-namespace ll {
-
-// Poll one wire vec until no word holds the sentinel (bounded like every other wait).
-template <int MODE>
-__device__ __forceinline__ void wait_vec(const CommDev& c, const uint8_t* p, dev::Wire<MODE>& w, bool pending) {
-  unsigned long long t0 = 0;
-  unsigned spins = 0;
-  while (pending) {
-    __nanosleep(40);
-    w = dev::wire_poll<MODE>(p, &pending);
-    if (pending && (++spins & 127u) == 0) {
-      const unsigned long long now = dev::globaltimer_ns();
-      if (t0 == 0) {
-        t0 = now;
-      } else if (now - t0 > c.timeout_ns) {
-        *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
-        __threadfence_system();
-        break;  // give up: results are undefined, but the GPU is not hung; the host sees the status word
-      }
-    }
-  }
-}
-
-}  // namespace ll
-
 template <int MODE, int W>
 __global__ void __launch_bounds__(kThreads, 1)
     k_ll(CommDev c, const __grid_constant__ Src src, void* buf, unsigned long long n, float scale) {
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
-  constexpr int U = Unroll<W>::kU;
+  constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
   const unsigned long long base_ll = (seq0 & 1u) ? c.ll_off[1] : c.ll_off[0];
   const bool aligned = buf_aligned<MODE>(buf);
@@ -73,8 +48,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   // the last that can have used this parity)
   if (threadIdx.x < W) {
     const int jj = threadIdx.x;
-    int p = c.rank + jj;
-    if (p >= W) p -= W;
+    const int p = slice_of<W>(c.rank, jj);
     if (blockIdx.x == 0)
       asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(reinterpret_cast<uint32_t*>(peer_sel(c, jj) + c.llflag_off) + c.rank), "r"(seq0)
                    : "memory");
@@ -91,8 +65,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V) x[u][jj] = load_src<MODE>(src, buf, gv * 8, n, aligned);
       }
@@ -102,8 +75,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        int j = c.rank + jj;
-        if (j >= W) j -= W;
+        const int j = slice_of<W>(c.rank, jj);
         const unsigned long long gv = j * Ls + v;
         if (v < Ls && gv < V)
           st_wire<MODE>(c.peer[jj] + my_recv + v * WVB, wire_no_sentinel<MODE>(compress<MODE>(x[u][jj], scale)));
@@ -143,7 +115,7 @@ __global__ void __launch_bounds__(kThreads, 1)
               for (int g = 0; g < G; ++g) {
                 if (r0 + g < W) {
                   uint8_t* p = mine + base_ll + (r0 + g) * c.slice_cap + v * WVB;
-                  if (pend[g]) ll::wait_vec<MODE>(c, p, w[g], true);
+                  if (pend[g]) wait_wire<MODE, 40, 128>(c, p, w[g]);
                   wire_reset<MODE>(p);  // back to "not written yet" for the collective after next
                   if (r0 + g == 0) s = widen<MODE>(w[g]);
                   else accumulate(s, widen<MODE>(w[g]));  // rank order, fp32
@@ -168,6 +140,8 @@ __global__ void __launch_bounds__(kThreads, 1)
             bool pend[G];
 #pragma unroll
             for (int g = 0; g < G; ++g) {
+              // slice_of<W>(c.rank, j0 + g), open-coded: the call moves ptxas's register allocation of k_ll at W = 3, 5,
+              // 6, 7 and 8 (spills appear or disappear), so both phase-3 rotations keep this form
               int j = c.rank + j0 + g;
               if (j >= W) j -= W;
               pend[g] = false;
@@ -181,7 +155,7 @@ __global__ void __launch_bounds__(kThreads, 1)
               const unsigned long long gv = j * Ls + v;
               if (j0 + g < W && v < Ls && gv < V) {
                 uint8_t* p = mine + base_ll + (static_cast<unsigned long long>(W) + j) * c.slice_cap + v * WVB;
-                if (pend[g]) ll::wait_vec<MODE>(c, p, w[g], true);
+                if (pend[g]) wait_wire<MODE, 40, 128>(c, p, w[g]);
                 store_out<MODE>(buf, gv * 8, n, aligned, w[g]);
                 wire_reset<MODE>(p);
               }

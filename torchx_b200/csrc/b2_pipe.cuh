@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   using namespace pl;
   constexpr int WVB = Wire<MODE>::kBytes;
-  constexpr int U = Unroll<W>::kU;
+  constexpr int U = vecs_per_trip(W);
   __shared__ uint32_t mail[2];  // [0]: chunks role A has finished, [1]: chunks role B has finished
   const uint32_t seq0 = op_begin(c);
   const uint32_t seq = seq0 * 4u + 1u;
@@ -154,8 +154,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           const unsigned long long v = v0 + static_cast<unsigned long long>(u) * kAD;
 #pragma unroll
           for (int jj = 0; jj < W; ++jj) {
-            int j = c.rank + jj;
-            if (j >= W) j -= W;
+            const int j = slice_of<W>(c.rank, jj);
             const unsigned long long gv = j * Ls + v;
             if (v < hi && gv < V) x[u][jj] = load_src<MODE>(src, buf, gv * 8, n, aligned);
           }
@@ -165,8 +164,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           const unsigned long long v = v0 + static_cast<unsigned long long>(u) * kAD;
 #pragma unroll
           for (int jj = 0; jj < W; ++jj) {
-            int j = c.rank + jj;
-            if (j >= W) j -= W;
+            const int j = slice_of<W>(c.rank, jj);
             const unsigned long long gv = j * Ls + v;
             if (v < hi && gv < V) {
               const Wire<MODE> w = compress<MODE>(x[u][jj], scale);
@@ -224,9 +222,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           for (int u = 0; u < U; ++u) {
             const unsigned long long v = v0 + static_cast<unsigned long long>(u) * kBD;
             if (v < hi && base + v < V) {
-              F8 s = widen<MODE>(w[u][0]);
-#pragma unroll
-              for (int r = 1; r < W; ++r) accumulate(s, widen<MODE>(w[u][r]));  // rank order, fp32
+              const F8 s = reduce_rank_order<MODE, W>(w[u]);
               st_wire<MODE>(mine + reduced + v * WVB, finalize<MODE>(s));
             }
           }
@@ -253,8 +249,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           const unsigned long long v = v0 + static_cast<unsigned long long>(u) * kCD;
 #pragma unroll
           for (int jj = 0; jj < W; ++jj) {
-            int j = c.rank + jj;
-            if (j >= W) j -= W;
+            const int j = slice_of<W>(c.rank, jj);
             const unsigned long long gv = j * Ls + v;
             pend[u][jj] = false;
             if (v < hi && gv < V) {
@@ -273,25 +268,8 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
             for (int jj = 0; jj < W; ++jj) {
               if (!pend[u][jj]) continue;
-              int j = c.rank + jj;
-              if (j >= W) j -= W;
-              const uint8_t* p = mine + nvls_out + j * c.slice_cap + v * WVB;
-              unsigned long long t0 = 0;
-              unsigned spins = 0;
-              bool pending = true;
-              while (pending) {
-                __nanosleep(64);
-                w[u][jj] = wire_poll<MODE>(p, &pending);
-                if (pending && (++spins & 63u) == 0) {
-                  const unsigned long long now = globaltimer_ns();
-                  if (t0 == 0) t0 = now;
-                  else if (now - t0 > c.timeout_ns) {
-                    *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
-                    __threadfence_system();
-                    break;
-                  }
-                }
-              }
+              const int j = slice_of<W>(c.rank, jj);
+              wait_wire<MODE, 64, 64>(c, mine + nvls_out + j * c.slice_cap + v * WVB, w[u][jj]);
             }
           }
         }
@@ -300,8 +278,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           const unsigned long long v = v0 + static_cast<unsigned long long>(u) * kCD;
 #pragma unroll
           for (int jj = 0; jj < W; ++jj) {
-            int j = c.rank + jj;
-            if (j >= W) j -= W;
+            const int j = slice_of<W>(c.rank, jj);
             const unsigned long long gv = j * Ls + v;
             if (v < hi && gv < V) {
               store_out<MODE>(buf, gv * 8, n, aligned, w[u][jj]);
