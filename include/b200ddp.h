@@ -14,8 +14,10 @@
  *                          CUDA-IPC exchange of one symmetric arena per rank over NVSwitch)
  *   b2_allreduce       <- the DDP bucket comm hook          torch/distributed/algorithms/ddp_comm_hooks/default_hooks.py:18-93
  *                         (`buf.to(bf16).div_(W)` -> ncclAllReduce(SUM) -> `buf.copy_()`, 4 launches; here ONE fused kernel)
- *                         and `dist.all_reduce`             torchx/schedulers/test/train.py:35,
+ *   b2_allreduce_op    <- `dist.all_reduce` of a metric      torchx/schedulers/test/train.py:35,
  *                                                           torchx/examples/apps/compute_world_size/module/util.py:37
+ *                         (both SUM an int64 one-hot tensor)
+ *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
  *   b2_broadcast       <- DDP init / per-forward buffer sync torch/nn/parallel/distributed.py:881-890, 2176-2243
  *   b2_barrier         <- dist.barrier()                     torchx/distributed/__init__.py:268,274,297,303
@@ -40,7 +42,8 @@
 extern "C" {
 #endif
 
-#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16 */
+#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op and b2_allgather, which only
+                            add symbols: a binding that needs them fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -208,6 +211,35 @@ int b2_allreduce_gather(b2_comm_t* comm, void* out, size_t n_elems, const b2_seg
 
 /* Broadcast `bytes` bytes at `buf` from rank `root` to every rank (bit-exact copy). */
 int b2_broadcast(b2_comm_t* comm, void* buf, size_t bytes, int root, void* stream);
+
+/*
+ * Exact collectives (DESIGN.md 2.4).  `dtype` is a B2_DT_*, `op` a B2_OP_*:
+ *   int32, int64                 SUM wraps (two's complement, modulo 2^32 / 2^64); MIN / MAX exact.
+ *   float32, bfloat16, float16   MIN / MAX exact: a NaN at any rank gives a NaN (its payload is unspecified but the same on
+ *                                every rank), otherwise IEEE 754-2019 minimum / maximum with -0.0 < +0.0; +-inf are
+ *                                ordinary values.
+ *                                SUM / AVG run b2_allreduce in B2_F32 / B2_BF16 / B2_F16 with scale 1 / (1/W) and
+ *                                B2_ALGO_AUTO: the rank-order fp32 sum with one final rounding (equal to NCCL at W = 2 only).
+ * The integer and MIN / MAX results are the same bits on every rank and do not depend on timing.  AVG on an integer
+ * dtype, any other op (PRODUCT, bitwise ...) and any other dtype are B2_EINVAL.
+ */
+#define B2_DT_INT32 0
+#define B2_DT_INT64 1
+#define B2_DT_FLOAT32 2
+#define B2_DT_BFLOAT16 3
+#define B2_DT_FLOAT16 4
+#define B2_OP_SUM 0
+#define B2_OP_AVG 1
+#define B2_OP_MIN 2
+#define B2_OP_MAX 3
+
+/* In place: buf[i] <- op_r buf_r[i] over `n_elems` elements (contract above).  n_elems == 0 is a no-op; W == 1 leaves
+ * `buf` as it is. */
+int b2_allreduce_op(b2_comm_t* comm, void* buf, size_t n_elems, int dtype, int op, void* stream);
+
+/* out[r*bytes .. (r+1)*bytes) <- rank r's `in` (bit-exact copy).  `in` may be exactly this rank's block of `out` (torch's
+ * in-place form); any other overlap of `in` and `out` is B2_EINVAL.  bytes == 0 is a no-op. */
+int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

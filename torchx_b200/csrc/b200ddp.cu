@@ -14,6 +14,7 @@
 //       - two-shot, piped : the same three phases as warp-specialised roles over K chunks            (b2_pipe.cuh)
 //       - NVLS, piped     : cast -> multimem.ld_reduce / multimem.st through the switch -> widen      (b2_pipe.cuh)
 //   * broadcast / barrier on the same fabric (DDP init + BN-buffer sync, dist.barrier()).
+//   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
 //
 // Memory model: every cross-GPU hand-off is  data stores -> bar.sync -> st.release.sys(flag)
 // on the producer and  ld.acquire.sys(flag) -> bar.sync -> data loads  on the consumer, with a
@@ -27,6 +28,7 @@
 #include "b2_kernels.cuh"
 #include "b2_pipe.cuh"
 #include "b2_ll.cuh"
+#include "b2_exact.cuh"
 #include "b2_vmm.h"
 
 #include <errno.h>
@@ -1102,6 +1104,123 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
     c->launches++;
     p += n;
     left -= n;
+  }
+  return B2_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+const char* dtype_name(int dtype) {
+  switch (dtype) {
+    case B2_DT_INT32: return "int32";
+    case B2_DT_INT64: return "int64";
+    case B2_DT_FLOAT32: return "float32";
+    case B2_DT_BFLOAT16: return "bfloat16";
+    case B2_DT_FLOAT16: return "float16";
+    default: return nullptr;
+  }
+}
+
+template <int DT>
+cudaError_t launch_reduce_exact(int op, const CommDev& d, int grid, void* buf, unsigned long long n, cudaStream_t s) {
+  switch (op) {
+    case B2_OP_SUM:
+      if constexpr (exact::DtypeTraits<DT>::kInt) k_reduce_exact<DT, B2_OP_SUM><<<grid, kThreads, 0, s>>>(d, buf, n);
+      else return cudaErrorInvalidValue;  // float SUM runs on the allreduce kernels
+      break;
+    case B2_OP_MIN:
+      k_reduce_exact<DT, B2_OP_MIN><<<grid, kThreads, 0, s>>>(d, buf, n);
+      break;
+    case B2_OP_MAX:
+      k_reduce_exact<DT, B2_OP_MAX><<<grid, kThreads, 0, s>>>(d, buf, n);
+      break;
+    default:
+      return cudaErrorInvalidValue;
+  }
+  return cudaGetLastError();
+}
+
+cudaError_t launch_reduce_exact(int dtype, int op, const CommDev& d, int grid, void* buf, unsigned long long n, cudaStream_t s) {
+  switch (dtype) {
+    case B2_DT_INT32: return launch_reduce_exact<B2_DT_INT32>(op, d, grid, buf, n, s);
+    case B2_DT_INT64: return launch_reduce_exact<B2_DT_INT64>(op, d, grid, buf, n, s);
+    case B2_DT_FLOAT32: return launch_reduce_exact<B2_DT_FLOAT32>(op, d, grid, buf, n, s);
+    case B2_DT_BFLOAT16: return launch_reduce_exact<B2_DT_BFLOAT16>(op, d, grid, buf, n, s);
+    case B2_DT_FLOAT16: return launch_reduce_exact<B2_DT_FLOAT16>(op, d, grid, buf, n, s);
+    default: return cudaErrorInvalidValue;
+  }
+}
+
+size_t dtype_bytes(int dtype) { return dtype == B2_DT_INT64 ? 8 : (dtype == B2_DT_BFLOAT16 || dtype == B2_DT_FLOAT16 ? 2 : 4); }
+
+}  // namespace
+
+extern "C" {
+
+int b2_allreduce_op(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, void* stream) {
+  const char* dt = dtype_name(dtype);
+  if (!dt) return fail(B2_EINVAL, "b2_allreduce_op: unknown dtype %d", dtype);
+  if (op != B2_OP_SUM && op != B2_OP_AVG && op != B2_OP_MIN && op != B2_OP_MAX)
+    return fail(B2_EINVAL, "b2_allreduce_op: unknown op %d", op);
+  const bool is_int = dtype == B2_DT_INT32 || dtype == B2_DT_INT64;
+  if (is_int && op == B2_OP_AVG) return fail(B2_EINVAL, "b2_allreduce_op: AVG needs a floating-point dtype, got %s", dt);
+  if (n_elems == 0) return B2_OK;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!buf) return fail(B2_EINVAL, "b2_allreduce_op: null buffer");
+  if (const int rc = check_not_poisoned(c)) return rc;
+  const int W = c->d.world;
+  if (W == 1) return B2_OK;
+  if (!is_int && (op == B2_OP_SUM || op == B2_OP_AVG)) {  // the rank-order fp32 sum of the gradient allreduce
+    const int mode = dtype == B2_DT_FLOAT32 ? B2_F32 : (dtype == B2_DT_BFLOAT16 ? B2_BF16 : B2_F16);
+    Src src = kNoSrc;
+    return allreduce_impl(c, src, buf, n_elems, mode, op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f, B2_ALGO_AUTO, stream);
+  }
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t eb = dtype_bytes(dtype);
+  const size_t cap = c->d.slice_cap / eb;  // elements one recv region holds (slice_cap is a multiple of 256 bytes)
+  uint8_t* p = static_cast<uint8_t*>(buf);
+  size_t left = n_elems;
+  while (left > 0) {
+    const size_t n = left < cap ? left : cap;
+    const int grid = grid_for(c, (n * eb + 15) / 16, 1);
+    const cudaError_t e = launch_reduce_exact(dtype, op, c->d, grid, p, n, s);
+    if (e != cudaSuccess) return fail(B2_ECUDA, "exact allreduce kernel launch: %s", cudaGetErrorString(e));
+    c->launches++;
+    p += n * eb;
+    left -= n;
+  }
+  return B2_OK;
+}
+
+int b2_allgather(b2_comm_t* c, void* out, const void* in, size_t bytes, void* stream) {
+  if (bytes == 0) return B2_OK;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!out || !in) return fail(B2_EINVAL, "b2_allgather: null buffer");
+  const int W = c->d.world;
+  const uintptr_t o = reinterpret_cast<uintptr_t>(out), i = reinterpret_cast<uintptr_t>(in);
+  const uintptr_t own = o + static_cast<uintptr_t>(c->d.rank) * bytes;
+  if (i != own && i < o + static_cast<uintptr_t>(W) * bytes && o < i + bytes)
+    return fail(B2_EINVAL, "b2_allgather: `in` overlaps `out` other than as this rank's block");
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (W == 1) {
+    if (i != own) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
+    return B2_OK;
+  }
+  const size_t cap = c->d.slice_cap;
+  size_t off = 0;
+  while (off < bytes) {
+    const size_t n = bytes - off < cap ? bytes - off : cap;
+    const int grid = grid_for(c, (n + 15) / 16, 1);
+    k_allgather<<<grid, kThreads, 0, s>>>(c->d, static_cast<uint8_t*>(out) + off, static_cast<const uint8_t*>(in) + off, n, bytes);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(B2_ECUDA, "all-gather kernel launch: %s", cudaGetErrorString(e));
+    c->launches++;
+    off += n;
   }
   return B2_OK;
 }

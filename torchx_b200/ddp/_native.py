@@ -45,6 +45,17 @@ B2_ALGO_TWOSHOT_LL = 5
 B2_CAP_VMM = 1
 B2_CAP_MULTICAST = 2
 
+B2_DT_INT32 = 0
+B2_DT_INT64 = 1
+B2_DT_FLOAT32 = 2
+B2_DT_BFLOAT16 = 3
+B2_DT_FLOAT16 = 4
+
+B2_OP_SUM = 0
+B2_OP_AVG = 1
+B2_OP_MIN = 2
+B2_OP_MAX = 3
+
 NVCC_FLAGS = [
     "-gencode",
     "arch=compute_90a,code=sm_90a",
@@ -78,6 +89,8 @@ SYMBOLS = [
     "b2_allreduce",
     "b2_allreduce_gather",
     "b2_broadcast",
+    "b2_allreduce_op",
+    "b2_allgather",
     "b2_barrier",
     "b2_local_pass",
 ]
@@ -161,6 +174,10 @@ def lib() -> ctypes.CDLL:
     L.b2_allreduce_gather.argtypes = [vp, vp, sz, ctypes.POINTER(B2Segment), i, i, f, i, vp]
     L.b2_broadcast.restype = i
     L.b2_broadcast.argtypes = [vp, vp, sz, i, vp]
+    L.b2_allreduce_op.restype = i
+    L.b2_allreduce_op.argtypes = [vp, vp, sz, i, i, vp]
+    L.b2_allgather.restype = i
+    L.b2_allgather.argtypes = [vp, vp, vp, sz, vp]
     L.b2_barrier.restype = i
     L.b2_barrier.argtypes = [vp, vp]
     L.b2_local_pass.restype = i

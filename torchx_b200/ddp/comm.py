@@ -22,6 +22,10 @@ _MODE_FOR = {
     ("bf16", "bf16"): N.B2_BF16,
     ("f16", "f16"): N.B2_F16,
 }
+# b2_allreduce_op: the dtypes and ops it takes (include/b200ddp.h)
+EXACT_DTYPES = {torch.int32: N.B2_DT_INT32, torch.int64: N.B2_DT_INT64, torch.float32: N.B2_DT_FLOAT32,
+                torch.bfloat16: N.B2_DT_BFLOAT16, torch.float16: N.B2_DT_FLOAT16}
+REDUCE_OPS = {"sum": N.B2_OP_SUM, "avg": N.B2_OP_AVG, "min": N.B2_OP_MIN, "max": N.B2_OP_MAX}
 ALGOS = {"auto": N.B2_ALGO_AUTO, "oneshot": N.B2_ALGO_ONESHOT, "twoshot": N.B2_ALGO_TWOSHOT, "twoshot_pipe": N.B2_ALGO_TWOSHOT_PIPE,
          "nvls": N.B2_ALGO_NVLS, "twoshot_ll": N.B2_ALGO_TWOSHOT_LL}
 
@@ -40,6 +44,18 @@ def mode_for(tensor: torch.Tensor, wire: str = "bf16") -> int:
     if key not in _MODE_FOR:
         raise ValueError(f"unsupported wire format {wire!r} for dtype {tensor.dtype}")
     return _MODE_FOR[key]
+
+
+def dtype_op_for(dtype: torch.dtype, op: str):
+    """(B2_DT_*, B2_OP_*) of an allreduce_op_ call.  TypeError for a dtype it does not take and for "avg" on an integer
+    dtype, ValueError for an op it does not know."""
+    if dtype not in EXACT_DTYPES:
+        raise TypeError(f"allreduce_op_: unsupported dtype {dtype}; expected int32, int64, float32, bfloat16 or float16")
+    if op not in REDUCE_OPS:
+        raise ValueError(f"allreduce_op_: unsupported op {op!r}; expected one of {sorted(REDUCE_OPS)}")
+    if op == "avg" and not dtype.is_floating_point:
+        raise TypeError(f"allreduce_op_: avg needs a floating-point tensor, got {dtype}")
+    return EXACT_DTYPES[dtype], REDUCE_OPS[op]
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream], device: int) -> int:
@@ -183,6 +199,28 @@ class Communicator:
         N.check(N.lib().b2_broadcast(self._h, ctypes.c_void_p(t.data_ptr()), t.numel() * t.element_size(), root,
                                      ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return t
+
+    def allreduce_op_(self, t: torch.Tensor, op: str = "sum", stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+        """In-place ``t <- op over ranks of t`` (include/b200ddp.h: b2_allreduce_op).  Integer SUM wraps, MIN / MAX are
+        exact; float SUM / AVG are the gradient allreduce with scale 1 / (1/W)."""
+        dt, code = dtype_op_for(t.dtype, op)
+        self._check_tensor(t)
+        N.check(N.lib().b2_allreduce_op(self._h, ctypes.c_void_p(t.data_ptr()), t.numel(), dt, code,
+                                        ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        return t
+
+    def allgather_(self, out: torch.Tensor, t: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+        """``out`` (world x the size of ``t``, same dtype) <- every rank's ``t`` in rank order (b2_allgather).  ``t`` may be
+        this rank's block of ``out``."""
+        if out.dtype != t.dtype:
+            raise TypeError(f"allgather_: out is {out.dtype}, input is {t.dtype}")
+        self._check_tensor(out)
+        self._check_tensor(t)
+        if out.numel() != self.world * t.numel():
+            raise ValueError(f"allgather_: out has {out.numel()} elements, needs {self.world} x {t.numel()}")
+        N.check(N.lib().b2_allgather(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()),
+                                     t.numel() * t.element_size(), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        return out
 
     def barrier(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         N.check(N.lib().b2_barrier(self._h, ctypes.c_void_p(_stream_ptr(stream, self.device))))

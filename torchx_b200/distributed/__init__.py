@@ -7,14 +7,14 @@ environment contract and barrier-ordered critical sections.  Two backends behind
   * a ``torch.distributed`` process group, exactly as the reference does (``init_pg("auto")`` -> nccl on GPU hosts, gloo
     otherwise) - this is what config #1 (CPU/gloo) and unmodified TorchX scripts use;
   * ``init_pg("b200")`` - the peer-buffer communicator from ``libb200ddp.so``: no TCP store, no NCCL.  ``barrier`` /
-    ``on_rank0_first`` then run on that fabric.
+    ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor`` and ``all_gather`` then run on that fabric.
 """
 from __future__ import annotations
 
 import os
 import warnings
 from contextlib import contextmanager
-from typing import Any, Iterator, Optional
+from typing import Any, Iterator, List, Optional
 
 import torch
 import torch.distributed as dist
@@ -118,6 +118,68 @@ def barrier() -> None:
         _COMM.check()  # a barrier kernel that gave up on a stalled peer must not let this rank into the critical section
     elif dist.is_initialized():
         dist.barrier()
+
+
+def _on_fabric() -> bool:
+    """The collectives below run on the native communicator: init_pg("b200") and no torch.distributed process group."""
+    return _COMM is not None and not dist.is_initialized()
+
+
+def _check_native_call(group: Any, async_op: bool) -> None:
+    if group is not None and group is not dist.group.WORLD:
+        raise NotImplementedError("the b200 communicator has no subgroups: pass group=None")
+    if async_op:
+        raise NotImplementedError("the b200 communicator has no work handles: collectives are ordered on the current stream")
+
+
+_REDUCE_OPS = ((dist.ReduceOp.SUM, "sum"), (dist.ReduceOp.AVG, "avg"), (dist.ReduceOp.MIN, "min"), (dist.ReduceOp.MAX, "max"))
+
+
+def reduce_op_name(op: Any) -> str:
+    """The allreduce_op_ name of a ``torch.distributed.ReduceOp``; ValueError for PRODUCT, the bitwise ops and the rest."""
+    for r, name in _REDUCE_OPS:
+        if op == r:
+            return name
+    raise ValueError(f"all_reduce on the b200 communicator supports SUM, AVG, MIN and MAX, not {op}")
+
+
+def all_reduce(tensor: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = None, async_op: bool = False) -> Any:
+    """``torch.distributed.all_reduce`` in place.  Under ``init_pg("b200")`` it runs on the native communicator on the current
+    stream: integer SUM (wrapping) and MIN / MAX are exact, float SUM / AVG are the rank-order fp32 sum (include/b200ddp.h).
+    With a process group it is ``torch.distributed.all_reduce``."""
+    if not _on_fabric():
+        return dist.all_reduce(tensor, op=op, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.allreduce_op_(tensor, reduce_op_name(op))
+    return None
+
+
+def all_gather_into_tensor(output_tensor: torch.Tensor, input_tensor: torch.Tensor, group: Any = None,
+                           async_op: bool = False) -> Any:
+    """``torch.distributed.all_gather_into_tensor``: ``output_tensor`` holds every rank's ``input_tensor`` in rank order
+    along its first dimension (or, flat, as world consecutive blocks)."""
+    if not _on_fabric():
+        return dist.all_gather_into_tensor(output_tensor, input_tensor, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.allgather_(output_tensor, input_tensor)
+    return None
+
+
+def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group: Any = None, async_op: bool = False) -> Any:
+    """``torch.distributed.all_gather``: ``tensor_list[r]`` <- rank r's ``tensor``."""
+    if not _on_fabric():
+        return dist.all_gather(tensor_list, tensor, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    if len(tensor_list) != _COMM.world:
+        raise ValueError(f"all_gather: tensor_list has {len(tensor_list)} tensors, world size is {_COMM.world}")
+    for t in tensor_list:
+        if t.dtype != tensor.dtype or t.numel() != tensor.numel():
+            raise ValueError(f"all_gather: every tensor of tensor_list must be {tensor.dtype} with {tensor.numel()} elements")
+    flat = torch.empty((_COMM.world,) + tuple(tensor.shape), dtype=tensor.dtype, device=tensor.device)
+    _COMM.allgather_(flat, tensor.contiguous())
+    for r, t in enumerate(tensor_list):
+        t.copy_(flat[r].view_as(t))
+    return None
 
 
 @contextmanager
