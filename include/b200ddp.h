@@ -18,6 +18,8 @@
  *                                                           torchx/examples/apps/compute_world_size/module/util.py:37
  *                         (both SUM an int64 one-hot tensor)
  *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
+ *   b2_batchnorm_stats <- torch's SyncBatchNorm forward: all_gather of (mean, invstd, count) + the count mask +
+ *                         batch_norm_gather_stats_with_counts (torch/nn/modules/_functions.py)
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
  *   b2_broadcast       <- DDP init / per-forward buffer sync torch/nn/parallel/distributed.py:881-890, 2176-2243
  *   b2_barrier         <- dist.barrier()                     torchx/distributed/__init__.py:268,274,297,303
@@ -42,8 +44,9 @@
 extern "C" {
 #endif
 
-#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op and b2_allgather, which only
-                            add symbols: a binding that needs them fails to resolve them against an older library */
+#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather and b2_batchnorm_stats,
+                            which only add symbols: a binding that needs them fails to resolve them against an older
+                            library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -240,6 +243,21 @@ int b2_allreduce_op(b2_comm_t* comm, void* buf, size_t n_elems, int dtype, int o
 /* out[r*bytes .. (r+1)*bytes) <- rank r's `in` (bit-exact copy).  `in` may be exactly this rank's block of `out` (torch's
  * in-place form); any other overlap of `in` and `out` is B2_EINVAL.  bytes == 0 is a no-op. */
 int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void* stream);
+
+/*
+ * SyncBatchNorm statistics: in place, mean[c] / invstd[c] <- the merge of every rank's (mean, invstd, count) over the ranks
+ * with count >= 1, in rank order, with the arithmetic of ATen's batch_norm_gather_stats_with_counts (DESIGN.md 2.4);
+ * running_mean / running_var (fp32, either may be NULL) updated in place; counts_out (W floats, may be NULL) <- every
+ * rank's count in rank order.  channels == 0 is a no-op.
+ * Replaces the statistics exchange of torch's SyncBatchNorm forward (torch/nn/modules/_functions.py: torch.cat of
+ * mean / invstd / count -> dist.all_gather_into_tensor -> the count >= 1 mask, a device-to-host sync -> counts.to() ->
+ * torch.batch_norm_gather_stats_with_counts) with one kernel and no host sync.  mean, invstd and the row's count must
+ * fit one stage region (B2_EINVAL otherwise); a negative or NaN count is B2_EINVAL.  At W == 1 the merge runs on this
+ * rank's row alone.
+ */
+int b2_batchnorm_stats(b2_comm_t* comm, float* mean, float* invstd, float count, size_t channels,
+                       float* running_mean, float* running_var, double momentum, double eps,
+                       float* counts_out, void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

@@ -15,6 +15,7 @@
 //       - NVLS, piped     : cast -> multimem.ld_reduce / multimem.st through the switch -> widen      (b2_pipe.cuh)
 //   * broadcast / barrier on the same fabric (DDP init + BN-buffer sync, dist.barrier()).
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
+//   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
 //
 // Memory model: every cross-GPU hand-off is  data stores -> bar.sync -> st.release.sys(flag)
 // on the producer and  ld.acquire.sys(flag) -> bar.sync -> data loads  on the consumer, with a
@@ -29,6 +30,7 @@
 #include "b2_pipe.cuh"
 #include "b2_ll.cuh"
 #include "b2_exact.cuh"
+#include "b2_bnstats.cuh"
 #include "b2_vmm.h"
 
 #include <errno.h>
@@ -1222,6 +1224,27 @@ int b2_allgather(b2_comm_t* c, void* out, const void* in, size_t bytes, void* st
     c->launches++;
     off += n;
   }
+  return B2_OK;
+}
+
+int b2_batchnorm_stats(b2_comm_t* c, float* mean, float* invstd, float count, size_t channels, float* running_mean,
+                       float* running_var, double momentum, double eps, float* counts_out, void* stream) {
+  if (channels == 0) return B2_OK;
+  if (!mean || !invstd) return fail(B2_EINVAL, "b2_batchnorm_stats: null mean or invstd");
+  if (!(count >= 0.0f)) return fail(B2_EINVAL, "b2_batchnorm_stats: count must be >= 0, got %g", static_cast<double>(count));
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  const size_t row = (2 * ((channels + 3) / 4) + 1) * 16;  // mean, invstd and the count, each in whole vecs
+  if (row > c->d.slice_cap)
+    return fail(B2_EINVAL, "b2_batchnorm_stats: %zu channels need a %zu-byte row, a stage region holds %llu", channels, row,
+                c->d.slice_cap);
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  // ATen's kernel takes eps and momentum as float parameters: the same double -> float conversion as at its launch
+  k_bn_stats<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(c->d, mean, invstd, count, channels, running_mean, running_var,
+                                                                    static_cast<float>(momentum), static_cast<float>(eps), counts_out);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm stats kernel launch: %s", cudaGetErrorString(e));
+  c->launches++;
   return B2_OK;
 }
 

@@ -86,6 +86,10 @@ class Communicator:
         self.rank = L.b2_comm_rank(self._h)
         self.world = L.b2_comm_world(self._h)
         self.device = L.b2_comm_device(self._h)
+        # The stream every collective of this communicator is issued on while an owner has one (the mini-DDP's comm stream:
+        # its bucket allreduces run there during backward).  A caller issuing another collective mid-backward enqueues it on
+        # this stream, between event waits in both directions, so the communicator stays one stream-ordered sequence.
+        self.ordered_stream: Optional[torch.cuda.Stream] = None
 
     # ---- construction --------------------------------------------------------------------------
     @classmethod
@@ -221,6 +225,32 @@ class Communicator:
         N.check(N.lib().b2_allgather(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()),
                                      t.numel() * t.element_size(), ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return out
+
+    def batchnorm_stats_(self, mean: torch.Tensor, invstd: torch.Tensor, count: float, running_mean: Optional[torch.Tensor] = None,
+                         running_var: Optional[torch.Tensor] = None, *, momentum: float, eps: float,
+                         counts_out: Optional[torch.Tensor] = None, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """SyncBatchNorm's statistics exchange (b2_batchnorm_stats): in place, ``mean`` / ``invstd`` (fp32, C channels) <-
+        the merge of every rank's (mean, invstd, count) with the arithmetic of torch.batch_norm_gather_stats_with_counts;
+        ``running_mean`` / ``running_var`` (fp32) updated in place when given; ``counts_out`` (fp32, world elements) <-
+        every rank's count in rank order."""
+        C = mean.numel()
+        given = [(name, t, n) for name, t, n in (("mean", mean, C), ("invstd", invstd, C), ("running_mean", running_mean, C),
+                                                 ("running_var", running_var, C), ("counts_out", counts_out, self.world))
+                 if t is not None]
+        for name, t, _ in given:
+            if t.dtype != torch.float32:
+                raise TypeError(f"batchnorm_stats_: {name} must be float32, got {t.dtype}")
+        for name, t, n in given:
+            self._check_tensor(t)
+            if t.numel() != n:
+                raise ValueError(f"batchnorm_stats_: {name} has {t.numel()} elements, expected {n}")
+
+        def ptr(t: Optional[torch.Tensor]) -> ctypes.c_void_p:
+            return ctypes.c_void_p(t.data_ptr() if t is not None else None)
+
+        N.check(N.lib().b2_batchnorm_stats(self._h, ptr(mean), ptr(invstd), ctypes.c_float(count), C, ptr(running_mean),
+                                           ptr(running_var), float(momentum), float(eps), ptr(counts_out),
+                                           ctypes.c_void_p(_stream_ptr(stream, self.device))))
 
     def barrier(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         N.check(N.lib().b2_barrier(self._h, ctypes.c_void_p(_stream_ptr(stream, self.device))))

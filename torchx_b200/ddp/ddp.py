@@ -114,6 +114,8 @@ class DistributedDataParallel(nn.Module):
             for p in b.params:
                 self._bucket_of[id(p)] = b
         self._comm_stream = torch.cuda.Stream(device=self.device)
+        # bucket allreduces run on this stream mid-backward: other collectives of the communicator (SyncBatchNorm) join it
+        self.comm.ordered_stream = self._comm_stream
         self._ready_event = torch.cuda.Event()
         self._next_bucket = 0
         self._callback_queued = False
