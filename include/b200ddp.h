@@ -18,6 +18,7 @@
  *                                                           torchx/examples/apps/compute_world_size/module/util.py:37
  *                         (both SUM an int64 one-hot tensor)
  *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
+ *   b2_reduce_scatter  <- `dist.reduce_scatter_tensor` / `dist.reduce_scatter`
  *   b2_batchnorm_stats <- torch's SyncBatchNorm forward: all_gather of (mean, invstd, count) + the count mask +
  *                         batch_norm_gather_stats_with_counts (torch/nn/modules/_functions.py)
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
@@ -44,9 +45,9 @@
 extern "C" {
 #endif
 
-#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather and b2_batchnorm_stats,
-                            which only add symbols: a binding that needs them fails to resolve them against an older
-                            library */
+#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats
+                            and b2_reduce_scatter, which only add symbols: a binding that needs them fails to resolve them
+                            against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -243,6 +244,14 @@ int b2_allreduce_op(b2_comm_t* comm, void* buf, size_t n_elems, int dtype, int o
 /* out[r*bytes .. (r+1)*bytes) <- rank r's `in` (bit-exact copy).  `in` may be exactly this rank's block of `out` (torch's
  * in-place form); any other overlap of `in` and `out` is B2_EINVAL.  bytes == 0 is a no-op. */
 int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void* stream);
+
+/* out[i] <- op_r in_r[rank*n_elems + i], i < n_elems; `in` holds W*n_elems elements (block r for rank r).  Same dtypes,
+ * ops and arithmetic contract as b2_allreduce_op: rank r's `out` is block r of what b2_allreduce_op of the same inputs
+ * leaves on every rank, bit for bit, except where that allreduce's B2_ALGO_AUTO picked B2_ALGO_NVLS (the reduce-scatter
+ * always sums in rank order).  `out` may be exactly this rank's block of `in` (the in-place form); any other overlap is
+ * B2_EINVAL.  n_elems == 0 is a no-op; at W == 1 it copies the block (nothing if in place).  Each rank sends and
+ * receives (W-1)/W of its input. */
+int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems, int dtype, int op, void* stream);
 
 /*
  * SyncBatchNorm statistics: in place, mean[c] / invstd[c] <- the merge of every rank's (mean, invstd, count) over the ranks

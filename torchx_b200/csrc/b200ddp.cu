@@ -15,6 +15,7 @@
 //       - NVLS, piped     : cast -> multimem.ld_reduce / multimem.st through the switch -> widen      (b2_pipe.cuh)
 //   * broadcast / barrier on the same fabric (DDP init + BN-buffer sync, dist.barrier()).
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
+//   * reduce-scatter with the allreduce's arithmetic: push-scatter, one barrier, reduce own block (b2_rs.cuh).
 //   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
 //
 // Memory model: every cross-GPU hand-off is  data stores -> bar.sync -> st.release.sys(flag)
@@ -30,6 +31,7 @@
 #include "b2_pipe.cuh"
 #include "b2_ll.cuh"
 #include "b2_exact.cuh"
+#include "b2_rs.cuh"
 #include "b2_bnstats.cuh"
 #include "b2_vmm.h"
 
@@ -386,6 +388,20 @@ cudaError_t launch_collective(const CommDev& d, const Src& src, int kind, int gr
       default:  // B2_ALGO_NVLS
         k_pipe<MODE, W, pl::kNvls><<<p.grid, kThreads, 0, s>>>(d, src, buf, n, scale, p.K, p.cell);
     }
+    return cudaGetLastError();
+  }
+}
+
+// The float reduce-scatter at the communicator's world size: instantiates k_reduce_scatter<MODE, W> for W = 2 ..
+// B2_MAX_WORLD.  Only the modes whose bucket is its own wire format (B2_F32 / B2_BF16 / B2_F16) have one.
+template <int MODE, int W = 2>
+cudaError_t launch_reduce_scatter(const CommDev& d, int grid, void* out, const void* in, unsigned long long n,
+                                  unsigned long long block, float scale, cudaStream_t s) {
+  if constexpr (W > B2_MAX_WORLD || ModeTraits<MODE>::kCastIn) {
+    return cudaErrorInvalidValue;
+  } else {
+    if (d.world != W) return launch_reduce_scatter<MODE, W + 1>(d, grid, out, in, n, block, scale, s);
+    k_reduce_scatter<MODE, W><<<grid, kThreads, 0, s>>>(d, out, in, n, block, scale);
     return cudaGetLastError();
   }
 }
@@ -1125,57 +1141,81 @@ const char* dtype_name(int dtype) {
   }
 }
 
-template <int DT>
-cudaError_t launch_reduce_exact(int op, const CommDev& d, int grid, void* buf, unsigned long long n, cudaStream_t s) {
+template <int DT, class F>
+bool with_exact_op_of(int op, F&& f) {
+  using Dt = std::integral_constant<int, DT>;
   switch (op) {
     case B2_OP_SUM:
-      if constexpr (exact::DtypeTraits<DT>::kInt) k_reduce_exact<DT, B2_OP_SUM><<<grid, kThreads, 0, s>>>(d, buf, n);
-      else return cudaErrorInvalidValue;  // float SUM runs on the allreduce kernels
-      break;
+      if constexpr (exact::DtypeTraits<DT>::kInt) {
+        f(Dt{}, std::integral_constant<int, B2_OP_SUM>{});
+        return true;
+      } else {
+        return false;  // float SUM runs on the allreduce kernels
+      }
     case B2_OP_MIN:
-      k_reduce_exact<DT, B2_OP_MIN><<<grid, kThreads, 0, s>>>(d, buf, n);
-      break;
+      f(Dt{}, std::integral_constant<int, B2_OP_MIN>{});
+      return true;
     case B2_OP_MAX:
-      k_reduce_exact<DT, B2_OP_MAX><<<grid, kThreads, 0, s>>>(d, buf, n);
-      break;
+      f(Dt{}, std::integral_constant<int, B2_OP_MAX>{});
+      return true;
     default:
-      return cudaErrorInvalidValue;
+      return false;
   }
-  return cudaGetLastError();
+}
+
+// The (dtype, op) pairs of the exact kernels: calls f(std::integral_constant<int, DT>{}, std::integral_constant<int, OP>{})
+// and returns true, or returns false for float SUM / AVG and anything unknown.  The only switch over them.
+template <class F>
+bool with_exact_op(int dtype, int op, F&& f) {
+  switch (dtype) {
+    case B2_DT_INT32: return with_exact_op_of<B2_DT_INT32>(op, f);
+    case B2_DT_INT64: return with_exact_op_of<B2_DT_INT64>(op, f);
+    case B2_DT_FLOAT32: return with_exact_op_of<B2_DT_FLOAT32>(op, f);
+    case B2_DT_BFLOAT16: return with_exact_op_of<B2_DT_BFLOAT16>(op, f);
+    case B2_DT_FLOAT16: return with_exact_op_of<B2_DT_FLOAT16>(op, f);
+    default: return false;
+  }
 }
 
 cudaError_t launch_reduce_exact(int dtype, int op, const CommDev& d, int grid, void* buf, unsigned long long n, cudaStream_t s) {
-  switch (dtype) {
-    case B2_DT_INT32: return launch_reduce_exact<B2_DT_INT32>(op, d, grid, buf, n, s);
-    case B2_DT_INT64: return launch_reduce_exact<B2_DT_INT64>(op, d, grid, buf, n, s);
-    case B2_DT_FLOAT32: return launch_reduce_exact<B2_DT_FLOAT32>(op, d, grid, buf, n, s);
-    case B2_DT_BFLOAT16: return launch_reduce_exact<B2_DT_BFLOAT16>(op, d, grid, buf, n, s);
-    case B2_DT_FLOAT16: return launch_reduce_exact<B2_DT_FLOAT16>(op, d, grid, buf, n, s);
-    default: return cudaErrorInvalidValue;
-  }
+  cudaError_t e = cudaErrorInvalidValue;
+  with_exact_op(dtype, op, [&](auto dt, auto o) {
+    k_reduce_exact<decltype(dt)::value, decltype(o)::value><<<grid, kThreads, 0, s>>>(d, buf, n);
+    e = cudaGetLastError();
+  });
+  return e;
 }
 
 size_t dtype_bytes(int dtype) { return dtype == B2_DT_INT64 ? 8 : (dtype == B2_DT_BFLOAT16 || dtype == B2_DT_FLOAT16 ? 2 : 4); }
+
+bool dtype_is_int(int dtype) { return dtype == B2_DT_INT32 || dtype == B2_DT_INT64; }
+
+// The B2_* mode of a float SUM / AVG: the gradient mode whose bucket has this dtype and is its own wire format.
+int sum_mode_for(int dtype) { return dtype == B2_DT_FLOAT32 ? B2_F32 : (dtype == B2_DT_BFLOAT16 ? B2_BF16 : B2_F16); }
+
+// Shared argument checks of b2_allreduce_op and b2_reduce_scatter, in their order: dtype, op, AVG on an integer dtype.
+int check_dtype_op(const char* fn, int dtype, int op) {
+  const char* dt = dtype_name(dtype);
+  if (!dt) return fail(B2_EINVAL, "%s: unknown dtype %d", fn, dtype);
+  if (op != B2_OP_SUM && op != B2_OP_AVG && op != B2_OP_MIN && op != B2_OP_MAX) return fail(B2_EINVAL, "%s: unknown op %d", fn, op);
+  if (dtype_is_int(dtype) && op == B2_OP_AVG) return fail(B2_EINVAL, "%s: AVG needs a floating-point dtype, got %s", fn, dt);
+  return B2_OK;
+}
 
 }  // namespace
 
 extern "C" {
 
 int b2_allreduce_op(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, void* stream) {
-  const char* dt = dtype_name(dtype);
-  if (!dt) return fail(B2_EINVAL, "b2_allreduce_op: unknown dtype %d", dtype);
-  if (op != B2_OP_SUM && op != B2_OP_AVG && op != B2_OP_MIN && op != B2_OP_MAX)
-    return fail(B2_EINVAL, "b2_allreduce_op: unknown op %d", op);
-  const bool is_int = dtype == B2_DT_INT32 || dtype == B2_DT_INT64;
-  if (is_int && op == B2_OP_AVG) return fail(B2_EINVAL, "b2_allreduce_op: AVG needs a floating-point dtype, got %s", dt);
+  if (const int rc = check_dtype_op("b2_allreduce_op", dtype, op)) return rc;
   if (n_elems == 0) return B2_OK;
   if (!c) return fail(B2_EINVAL, "null communicator");
   if (!buf) return fail(B2_EINVAL, "b2_allreduce_op: null buffer");
   if (const int rc = check_not_poisoned(c)) return rc;
   const int W = c->d.world;
   if (W == 1) return B2_OK;
-  if (!is_int && (op == B2_OP_SUM || op == B2_OP_AVG)) {  // the rank-order fp32 sum of the gradient allreduce
-    const int mode = dtype == B2_DT_FLOAT32 ? B2_F32 : (dtype == B2_DT_BFLOAT16 ? B2_BF16 : B2_F16);
+  if (!dtype_is_int(dtype) && (op == B2_OP_SUM || op == B2_OP_AVG)) {  // the rank-order fp32 sum of the gradient allreduce
+    const int mode = sum_mode_for(dtype);
     Src src = kNoSrc;
     return allreduce_impl(c, src, buf, n_elems, mode, op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f, B2_ALGO_AUTO, stream);
   }
@@ -1221,6 +1261,56 @@ int b2_allgather(b2_comm_t* c, void* out, const void* in, size_t bytes, void* st
     k_allgather<<<grid, kThreads, 0, s>>>(c->d, static_cast<uint8_t*>(out) + off, static_cast<const uint8_t*>(in) + off, n, bytes);
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(B2_ECUDA, "all-gather kernel launch: %s", cudaGetErrorString(e));
+    c->launches++;
+    off += n;
+  }
+  return B2_OK;
+}
+
+int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, int dtype, int op, void* stream) {
+  if (const int rc = check_dtype_op("b2_reduce_scatter", dtype, op)) return rc;
+  if (n_elems == 0) return B2_OK;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!out || !in) return fail(B2_EINVAL, "b2_reduce_scatter: null buffer");
+  const int W = c->d.world;
+  const size_t eb = dtype_bytes(dtype);
+  const size_t bytes = n_elems * eb;  // one block
+  const uintptr_t o = reinterpret_cast<uintptr_t>(out), i = reinterpret_cast<uintptr_t>(in);
+  const uintptr_t own = i + static_cast<uintptr_t>(c->d.rank) * bytes;
+  if (o != own && o < i + static_cast<uintptr_t>(W) * bytes && i < o + bytes)
+    return fail(B2_EINVAL, "b2_reduce_scatter: `out` overlaps `in` other than as this rank's block");
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (W == 1) {
+    if (o != own) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
+    return B2_OK;
+  }
+  const bool sum = !dtype_is_int(dtype) && (op == B2_OP_SUM || op == B2_OP_AVG);
+  const int mode = sum_mode_for(dtype);
+  // elements of a block one recv region holds: a whole number of vecs in either case (slice_cap is a multiple of 256 bytes)
+  const size_t cap = sum ? c->d.slice_cap / wire_vec_bytes(mode) * 8 : c->d.slice_cap / eb;
+  const float scale = op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f;
+  uint8_t* po = static_cast<uint8_t*>(out);
+  const uint8_t* pi = static_cast<const uint8_t*>(in);
+  size_t off = 0;
+  while (off < n_elems) {
+    const size_t n = n_elems - off < cap ? n_elems - off : cap;
+    cudaError_t e = cudaErrorInvalidValue;  // never guess a mode
+    if (sum) {
+      const int grid = grid_for(c, (n + 7) / 8, vecs_per_trip(W));
+      with_mode(mode, [&](auto m) {
+        e = launch_reduce_scatter<decltype(m)::value>(c->d, grid, po + off * eb, pi + off * eb, n, n_elems, scale, s);
+      });
+    } else {
+      const int grid = grid_for(c, (n * eb + 15) / 16, 1);
+      with_exact_op(dtype, op, [&](auto dt, auto oc) {
+        k_reduce_scatter_exact<decltype(dt)::value, decltype(oc)::value><<<grid, kThreads, 0, s>>>(c->d, po + off * eb, pi + off * eb,
+                                                                                                 n, n_elems);
+        e = cudaGetLastError();
+      });
+    }
+    if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
     c->launches++;
     off += n;
   }

@@ -91,6 +91,7 @@ SYMBOLS = [
     "b2_broadcast",
     "b2_allreduce_op",
     "b2_allgather",
+    "b2_reduce_scatter",
     "b2_batchnorm_stats",
     "b2_barrier",
     "b2_local_pass",
@@ -179,6 +180,8 @@ def lib() -> ctypes.CDLL:
     L.b2_allreduce_op.argtypes = [vp, vp, sz, i, i, vp]
     L.b2_allgather.restype = i
     L.b2_allgather.argtypes = [vp, vp, vp, sz, vp]
+    L.b2_reduce_scatter.restype = i
+    L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
     L.b2_batchnorm_stats.restype = i
     L.b2_batchnorm_stats.argtypes = [vp, vp, vp, f, sz, vp, vp, ctypes.c_double, ctypes.c_double, vp, vp]
     L.b2_barrier.restype = i

@@ -46,15 +46,15 @@ def mode_for(tensor: torch.Tensor, wire: str = "bf16") -> int:
     return _MODE_FOR[key]
 
 
-def dtype_op_for(dtype: torch.dtype, op: str):
-    """(B2_DT_*, B2_OP_*) of an allreduce_op_ call.  TypeError for a dtype it does not take and for "avg" on an integer
-    dtype, ValueError for an op it does not know."""
+def dtype_op_for(dtype: torch.dtype, op: str, fn: str = "allreduce_op_"):
+    """(B2_DT_*, B2_OP_*) of an allreduce_op_ or reduce_scatter_ call.  TypeError for a dtype it does not take and for
+    "avg" on an integer dtype, ValueError for an op it does not know."""
     if dtype not in EXACT_DTYPES:
-        raise TypeError(f"allreduce_op_: unsupported dtype {dtype}; expected int32, int64, float32, bfloat16 or float16")
+        raise TypeError(f"{fn}: unsupported dtype {dtype}; expected int32, int64, float32, bfloat16 or float16")
     if op not in REDUCE_OPS:
-        raise ValueError(f"allreduce_op_: unsupported op {op!r}; expected one of {sorted(REDUCE_OPS)}")
+        raise ValueError(f"{fn}: unsupported op {op!r}; expected one of {sorted(REDUCE_OPS)}")
     if op == "avg" and not dtype.is_floating_point:
-        raise TypeError(f"allreduce_op_: avg needs a floating-point tensor, got {dtype}")
+        raise TypeError(f"{fn}: avg needs a floating-point tensor, got {dtype}")
     return EXACT_DTYPES[dtype], REDUCE_OPS[op]
 
 
@@ -224,6 +224,22 @@ class Communicator:
             raise ValueError(f"allgather_: out has {out.numel()} elements, needs {self.world} x {t.numel()}")
         N.check(N.lib().b2_allgather(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()),
                                      t.numel() * t.element_size(), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        return out
+
+    def reduce_scatter_(self, out: torch.Tensor, t: torch.Tensor, op: str = "sum",
+                        stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+        """``out`` <- block ``rank`` of the ``allreduce_op_`` of ``t`` (world x the size of ``out``, same dtype) over the ranks
+        (include/b200ddp.h: b2_reduce_scatter): the same bits that allreduce leaves there, moving only (W-1)/W of ``t``.
+        ``out`` may be this rank's block of ``t``."""
+        dt, code = dtype_op_for(t.dtype, op, "reduce_scatter_")
+        if out.dtype != t.dtype:
+            raise TypeError(f"reduce_scatter_: out is {out.dtype}, input is {t.dtype}")
+        if t.numel() != self.world * out.numel():
+            raise ValueError(f"reduce_scatter_: input has {t.numel()} elements, needs {self.world} x {out.numel()}")
+        self._check_tensor(out)
+        self._check_tensor(t)
+        N.check(N.lib().b2_reduce_scatter(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()), out.numel(), dt,
+                                          code, ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return out
 
     def batchnorm_stats_(self, mean: torch.Tensor, invstd: torch.Tensor, count: float, running_mean: Optional[torch.Tensor] = None,

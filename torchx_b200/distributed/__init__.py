@@ -7,7 +7,8 @@ environment contract and barrier-ordered critical sections.  Two backends behind
   * a ``torch.distributed`` process group, exactly as the reference does (``init_pg("auto")`` -> nccl on GPU hosts, gloo
     otherwise) - this is what config #1 (CPU/gloo) and unmodified TorchX scripts use;
   * ``init_pg("b200")`` - the peer-buffer communicator from ``libb200ddp.so``: no TCP store, no NCCL.  ``barrier`` /
-    ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor`` and ``all_gather`` then run on that fabric.
+    ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor``, ``all_gather``, ``reduce_scatter_tensor``,
+    ``reduce_scatter`` and ``broadcast`` then run on that fabric.
 """
 from __future__ import annotations
 
@@ -140,7 +141,7 @@ def reduce_op_name(op: Any) -> str:
     for r, name in _REDUCE_OPS:
         if op == r:
             return name
-    raise ValueError(f"all_reduce on the b200 communicator supports SUM, AVG, MIN and MAX, not {op}")
+    raise ValueError(f"a reduction on the b200 communicator supports SUM, AVG, MIN and MAX, not {op}")
 
 
 def all_reduce(tensor: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = None, async_op: bool = False) -> Any:
@@ -179,6 +180,43 @@ def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group: Any
     _COMM.allgather_(flat, tensor.contiguous())
     for r, t in enumerate(tensor_list):
         t.copy_(flat[r].view_as(t))
+    return None
+
+
+def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = None,
+                          async_op: bool = False) -> Any:
+    """``torch.distributed.reduce_scatter_tensor``: ``input`` holds world blocks of ``output``'s size (along its first
+    dimension, or flat); rank r's ``output`` <- the reduction over ranks of block r.  Under ``init_pg("b200")`` that is
+    block r of what ``all_reduce`` with the same op leaves, bit for bit, at (W-1)/W of the input's bytes per rank."""
+    if not _on_fabric():
+        return dist.reduce_scatter_tensor(output, input, op=op, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.reduce_scatter_(output, input, reduce_op_name(op))
+    return None
+
+
+def reduce_scatter(output: torch.Tensor, input_list: List[torch.Tensor], op: Any = dist.ReduceOp.SUM, group: Any = None,
+                   async_op: bool = False) -> Any:
+    """``torch.distributed.reduce_scatter``: rank r's ``output`` <- the reduction over ranks of their ``input_list[r]``."""
+    if not _on_fabric():
+        return dist.reduce_scatter(output, input_list, op=op, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    name = reduce_op_name(op)
+    if len(input_list) != _COMM.world:
+        raise ValueError(f"reduce_scatter: input_list has {len(input_list)} tensors, world size is {_COMM.world}")
+    for t in input_list:
+        if t.dtype != output.dtype or t.numel() != output.numel():
+            raise ValueError(f"reduce_scatter: every tensor of input_list must be {output.dtype} with {output.numel()} elements")
+    _COMM.reduce_scatter_(output, torch.cat([t.reshape(-1) for t in input_list]), name)
+    return None
+
+
+def broadcast(tensor: torch.Tensor, src: int, group: Any = None, async_op: bool = False) -> Any:
+    """``torch.distributed.broadcast`` in place: every rank's ``tensor`` <- rank ``src``'s, bit for bit."""
+    if not _on_fabric():
+        return dist.broadcast(tensor, src, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.broadcast_(tensor, root=src)
     return None
 
 
