@@ -45,9 +45,9 @@
 extern "C" {
 #endif
 
-#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats
-                            and b2_reduce_scatter, which only add symbols: a binding that needs them fails to resolve them
-                            against an older library */
+#define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
+                            b2_reduce_scatter and b2_bn_*_elemt, which only add symbols: a binding that needs them fails to resolve
+                            them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -267,6 +267,25 @@ int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems
 int b2_batchnorm_stats(b2_comm_t* comm, float* mean, float* invstd, float count, size_t channels,
                        float* running_mean, float* running_var, double momentum, double eps,
                        float* counts_out, void* stream);
+
+/*
+ * The elementwise passes of training-mode BatchNorm2d on channels-last activations (no communicator; DESIGN.md 2.3 / 2.4).
+ * The data is the row-major [rows, channels] view of an NHWC-contiguous tensor (rows = N*H*W); x, y, dy and dx are `dtype`
+ * (B2_DT_BFLOAT16, the one format whose torch BatchNorm runs ATen's own kernels rather than cuDNN's), 16-byte aligned; every
+ * other array is float32 [channels].  The reductions are ATen's
+ * (torch.batch_norm_update_stats, torch.batch_norm_backward_reduce) and the arithmetic here is ATen's, expression for
+ * expression, so the results are the bits ATen's own BatchNorm computes.  eps is converted to float as ATen's launch does.
+ * No call allocates or synchronises the host.  channels % 8 != 0, rows < 2, an unknown dtype, a null or a misaligned
+ * pointer is B2_EINVAL.
+ */
+/* save_invstd <- rsqrt(var + eps) (var: the biased batch variance); y <- weight * (x - mean) * save_invstd + bias. */
+int b2_bn_forward_elemt(const void* x, void* y, size_t rows, size_t channels, int dtype, const float* weight, const float* bias,
+                        const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream);
+
+/* dx <- (dy - sum_dy / rows - (x - mean) * invstd^2 * sum_dy_xmu / rows) * invstd * weight. */
+int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
+                         const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, int device,
+                         void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

@@ -17,6 +17,7 @@
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
 //   * reduce-scatter with the allreduce's arithmetic: push-scatter, one barrier, reduce own block (b2_rs.cuh).
 //   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
+//   * the elementwise passes of training-mode BatchNorm2d on channels-last bf16 activations (b2_bn.cuh).
 //
 // Memory model: every cross-GPU hand-off is  data stores -> bar.sync -> st.release.sys(flag)
 // on the producer and  ld.acquire.sys(flag) -> bar.sync -> data loads  on the consumer, with a
@@ -33,6 +34,7 @@
 #include "b2_exact.cuh"
 #include "b2_rs.cuh"
 #include "b2_bnstats.cuh"
+#include "b2_bn.cuh"
 #include "b2_vmm.h"
 
 #include <errno.h>
@@ -1335,6 +1337,78 @@ int b2_batchnorm_stats(b2_comm_t* c, float* mean, float* invstd, float count, si
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm stats kernel launch: %s", cudaGetErrorString(e));
   c->launches++;
+  return B2_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+constexpr int kBnFwdUnroll = 4;  // x vecs in flight per thread (forward elementwise)
+constexpr int kBnBwdUnroll = 2;  // x and dy vecs: 2 x 2 in flight per thread (backward elementwise)
+
+int bn_check_shape(const char* fn, int dtype, size_t M, size_t C) {
+  if (dtype != B2_DT_BFLOAT16) return fail(B2_EINVAL, "%s: dtype %d is not B2_DT_BFLOAT16", fn, dtype);
+  if (C == 0 || C % 8 != 0) return fail(B2_EINVAL, "%s: channels=%zu must be a positive multiple of 8", fn, C);
+  if (M < 2) return fail(B2_EINVAL, "%s: rows=%zu, batch statistics need at least 2", fn, M);
+  return B2_OK;
+}
+
+struct BnPtr {
+  const char* name;
+  const void* p;
+  unsigned align;
+};
+
+int bn_check_ptrs(const char* fn, std::initializer_list<BnPtr> ps) {
+  for (const BnPtr& q : ps) {
+    if (!q.p) return fail(B2_EINVAL, "%s: null %s", fn, q.name);
+    if (reinterpret_cast<uintptr_t>(q.p) % q.align != 0)
+      return fail(B2_EINVAL, "%s: %s is not %u-byte aligned", fn, q.name, q.align);
+  }
+  return B2_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b2_bn_forward_elemt(const void* x, void* y, size_t rows, size_t channels, int dtype, const float* weight, const float* bias,
+                        const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream) {
+  static const char* fn = "b2_bn_forward_elemt";
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"y", y, 16}, {"weight", weight, 4}, {"bias", bias, 4}, {"mean", mean, 4},
+                                        {"var", var, 4}, {"save_invstd", save_invstd, 4}}))
+    return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bn::Plan p = bn::plan(rows, channels, sm_count(device), kBnFwdUnroll);
+  // ATen converts eps to float at its launch (acc_t); so does this call
+  k_bn2d_norm<kBnFwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y), rows,
+                                                                         channels, p, mean, var, static_cast<float>(eps), save_invstd,
+                                                                         weight, bias);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm forward kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
+                         const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, int device,
+                         void* stream) {
+  static const char* fn = "b2_bn_backward_elemt";
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}, {"dx", dx, 16}, {"weight", weight, 4}, {"mean", mean, 4},
+                                        {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4}, {"sum_dy_xmu", sum_dy_xmu, 4}}))
+    return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bn::Plan p = bn::plan(rows, channels, sm_count(device), kBnBwdUnroll);
+  // ATen's norm_fct: 1 / count in double, converted to float
+  k_bn2d_bwd_elemt<kBnBwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(
+      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), static_cast<uint16_t*>(dx), rows, channels, p, mean, invstd,
+      weight, sum_dy, sum_dy_xmu, static_cast<float>(1.0 / static_cast<double>(rows)));
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 

@@ -93,6 +93,8 @@ SYMBOLS = [
     "b2_allgather",
     "b2_reduce_scatter",
     "b2_batchnorm_stats",
+    "b2_bn_forward_elemt",
+    "b2_bn_backward_elemt",
     "b2_barrier",
     "b2_local_pass",
 ]
@@ -184,6 +186,10 @@ def lib() -> ctypes.CDLL:
     L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
     L.b2_batchnorm_stats.restype = i
     L.b2_batchnorm_stats.argtypes = [vp, vp, vp, f, sz, vp, vp, ctypes.c_double, ctypes.c_double, vp, vp]
+    L.b2_bn_forward_elemt.restype = i
+    L.b2_bn_forward_elemt.argtypes = [vp, vp, sz, sz, i, vp, vp, vp, vp, ctypes.c_double, vp, i, vp]
+    L.b2_bn_backward_elemt.restype = i
+    L.b2_bn_backward_elemt.argtypes = [vp, vp, vp, sz, sz, i, vp, vp, vp, vp, vp, i, vp]
     L.b2_barrier.restype = i
     L.b2_barrier.argtypes = [vp, vp]
     L.b2_local_pass.restype = i

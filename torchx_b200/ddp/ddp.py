@@ -11,7 +11,9 @@ a 1 MiB first bucket, per-forward buffer broadcast, ``no_sync``, ``module.``-pre
     (a device pointer table per bucket) and writes the averaged values into the persistent flat bucket, which
     ``param.grad`` aliases afterwards (gradient_as_bucket_view semantics) - the Reducer's copy-in pass
     (reducer.cpp mark_variable_ready_dense) and its 8 bytes per element are gone;
-  * the layout is the steady-state one from iteration 0 (no rebuild pass).
+  * the layout is the steady-state one from iteration 0 (no rebuild pass);
+  * the wrapped module's ``nn.BatchNorm2d`` layers become ``torchx_b200.nn.BatchNorm2d``: channels-last bf16 / fp16
+    training runs on bandwidth-bound native kernels, every other input on ATen as before (DESIGN.md 2.5).
 """
 from __future__ import annotations
 
@@ -123,6 +125,10 @@ class DistributedDataParallel(nn.Module):
         self.copied_in_buckets = 0   # buckets that needed the multi-tensor copy-in (zero-copy not applicable), for tests / bench
         self.gathered_buckets = 0    # buckets whose gradients were read in place by the kernel
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad_ready) for p in self._params]
+        # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen
+        from torchx_b200.nn.bn2d import convert_batchnorm
+
+        convert_batchnorm(module)
         self._sync_module_states()
 
     # ---- construction-time / per-forward state sync (reference: distributed.py:881-890, 2176-2243) ----
