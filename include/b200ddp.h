@@ -19,6 +19,7 @@
  *                         (both SUM an int64 one-hot tensor)
  *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
  *   b2_reduce_scatter  <- `dist.reduce_scatter_tensor` / `dist.reduce_scatter`
+ *   b2_alltoall, b2_alltoall_max_bytes <- `dist.all_to_all_single` / `dist.all_to_all`
  *   b2_batchnorm_stats <- torch's SyncBatchNorm forward: all_gather of (mean, invstd, count) + the count mask +
  *                         batch_norm_gather_stats_with_counts (torch/nn/modules/_functions.py)
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
@@ -46,8 +47,8 @@ extern "C" {
 #endif
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
-                            b2_reduce_scatter and b2_bn_*_elemt, which only add symbols: a binding that needs them fails to resolve
-                            them against an older library */
+                            b2_reduce_scatter, b2_bn_*_elemt and b2_alltoall*, which only add symbols: a binding that needs them
+                            fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -160,9 +161,11 @@ int b2_auto_algo(int world, int mode, size_t n_elems, int has_multicast);
 int b2_comm_set_param(b2_comm_t* comm, const char* name, long long value);
 
 /*
- * Non-blocking health check: B2_OK, or B2_ETIMEOUT if any kernel of this communicator gave up
- * waiting for a peer (its output is then undefined).  Reads a host-mapped status word; does not
- * synchronise the device.
+ * Non-blocking health check: B2_OK, B2_ETIMEOUT if any kernel of this communicator gave up
+ * waiting for a peer (its output is then undefined), or B2_EINVAL if an all-to-all's split sizes
+ * disagreed across ranks or exceeded the per-pair limit (see b2_alltoall).  Reads a host-mapped
+ * status word; does not synchronise the device.  Either code poisons the communicator: every later
+ * collective returns B2_ESTATE.
  */
 int b2_comm_status(const b2_comm_t* comm);
 
@@ -252,6 +255,31 @@ int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void*
  * B2_EINVAL.  n_elems == 0 is a no-op; at W == 1 it copies the block (nothing if in place).  Each rank sends and
  * receives (W-1)/W of its input. */
 int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems, int dtype, int op, void* stream);
+
+/*
+ * All-to-all, a bit-exact copy of bytes (any dtype): out[r] <- the recv_bytes[r] bytes rank r sends this rank, in[j] is what
+ * goes to rank j (send_bytes[j] bytes).  The four arrays are HOST arrays of W entries indexed by rank, copied into the kernel
+ * parameters by the call; a pointer whose count is 0 may be NULL.  No `out` range may overlap another `out` range or any
+ * `in` range (there is no in-place form).  One launch per call whatever the sizes, so each (sender, receiver) pair of
+ * distinct ranks carries at most b2_alltoall_max_bytes(comm) bytes (a rank's block to itself is copied directly and has
+ * no limit).  Each rank sends and receives (W-1)/W of its data when the splits are even.
+ *   - A null communicator or array, a null pointer with a non-zero count, or an overlap: B2_EINVAL before anything is
+ *     launched; a poisoned communicator: B2_ESTATE.
+ *   - A pair over the limit: its sender's and its receiver's calls return B2_EINVAL, but still launch so that no rank
+ *     waits for them; every rank's kernel then gives up the exchange, writes no output and records B2_EINVAL for
+ *     b2_comm_status, which poisons every rank's communicator.
+ *   - recv_bytes[r] different from what rank r sends this rank (send_bytes[rank] vs recv_bytes[rank] included): only this
+ *     rank's kernel sees it.  It writes none of this rank's outputs and records B2_EINVAL, poisoning this rank's
+ *     communicator; the other ranks complete normally.  At W == 1 the call returns B2_EINVAL instead.
+ * At W > 1 a rank whose counts are all 0 still takes part (the other ranks' barriers include it).  At W == 1 the call is
+ * one device-to-device copy.
+ */
+int b2_alltoall(b2_comm_t* comm, void* const* out, const size_t* recv_bytes, const void* const* in, const size_t* send_bytes,
+                void* stream);
+
+/* The most bytes one rank may send another in one b2_alltoall: a stage region less its 16-byte count header (the stage
+ * size is b2_comm_create's stage_bytes, default 512 MiB, divided into W + 1 regions).  0 for a null communicator. */
+size_t b2_alltoall_max_bytes(const b2_comm_t* comm);
 
 /*
  * SyncBatchNorm statistics: in place, mean[c] / invstd[c] <- the merge of every rank's (mean, invstd, count) over the ranks

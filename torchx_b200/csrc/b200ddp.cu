@@ -16,6 +16,7 @@
 //   * broadcast / barrier on the same fabric (DDP init + BN-buffer sync, dist.barrier()).
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
 //   * reduce-scatter with the allreduce's arithmetic: push-scatter, one barrier, reduce own block (b2_rs.cuh).
+//   * all-to-all with any split sizes: push each block behind a count header, one barrier, copy out (b2_a2a.cuh).
 //   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
 //   * the elementwise passes of training-mode BatchNorm2d on channels-last bf16 activations (b2_bn.cuh).
 //
@@ -33,6 +34,7 @@
 #include "b2_ll.cuh"
 #include "b2_exact.cuh"
 #include "b2_rs.cuh"
+#include "b2_a2a.cuh"
 #include "b2_bnstats.cuh"
 #include "b2_bn.cuh"
 #include "b2_vmm.h"
@@ -512,10 +514,15 @@ bool wait_count(std::atomic<int>& ctr, int target, std::atomic<int>* abort_flag,
   return true;
 }
 
-// A kernel that gave up waiting for a peer leaves the communicator's buffers and counters in an unknown state.
+// What a kernel records in the status word: B2_ETIMEOUT (a peer wait gave up) or B2_EINVAL (k_alltoall), which says:
+constexpr const char* kA2aStatusText = "an all-to-all's split sizes disagreed across ranks or exceeded the per-pair limit";
+
+// A kernel that gave up waiting for a peer leaves the communicator's buffers and counters in an unknown state.  An
+// all-to-all that gave up its exchange leaves them consistent, but the outputs of that call are not written.
 int check_not_poisoned(const b2_comm* c) {
-  if (*reinterpret_cast<volatile uint32_t*>(c->status_host) != 0)
-    return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
+  const uint32_t s = *reinterpret_cast<volatile uint32_t*>(c->status_host);
+  if (s == static_cast<uint32_t>(-B2_EINVAL)) return fail(B2_ESTATE, "communicator poisoned: %s", kA2aStatusText);
+  if (s != 0) return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
   return B2_OK;
 }
 
@@ -991,8 +998,8 @@ int b2_comm_status(const b2_comm_t* c) {
   if (!c) return fail(B2_EINVAL, "null communicator");
   const uint32_t s = *reinterpret_cast<volatile uint32_t*>(c->status_host);
   if (s == 0) return B2_OK;
-  return fail(-static_cast<int>(s), "rank %d: a kernel gave up waiting for a peer (code %d)", c->d.rank,
-              -static_cast<int>(s));
+  return fail(-static_cast<int>(s), "rank %d: %s (code %d)", c->d.rank,
+              s == static_cast<uint32_t>(-B2_EINVAL) ? kA2aStatusText : "a kernel gave up waiting for a peer", -static_cast<int>(s));
 }
 
 uint64_t b2_comm_launch_count(const b2_comm_t* c) { return c ? c->launches : 0; }
@@ -1317,6 +1324,59 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
     off += n;
   }
   return B2_OK;
+}
+
+size_t b2_alltoall_max_bytes(const b2_comm_t* c) { return c ? c->d.slice_cap - kA2aHeaderBytes : 0; }
+
+int b2_alltoall(b2_comm_t* c, void* const* out, const size_t* recv_bytes, const void* const* in, const size_t* send_bytes,
+                void* stream) {
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!out || !recv_bytes || !in || !send_bytes) return fail(B2_EINVAL, "b2_alltoall: null array");
+  const int W = c->d.world, me = c->d.rank;
+  for (int r = 0; r < W; ++r) {
+    if (!out[r] && recv_bytes[r]) return fail(B2_EINVAL, "b2_alltoall: out[%d] is null but recv_bytes[%d] = %zu", r, r, recv_bytes[r]);
+    if (!in[r] && send_bytes[r]) return fail(B2_EINVAL, "b2_alltoall: in[%d] is null but send_bytes[%d] = %zu", r, r, send_bytes[r]);
+  }
+  const auto overlap = [](const void* p, size_t n, const void* q, size_t m) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+    return n && m && a < b + m && b < a + n;
+  };
+  for (int r = 0; r < W; ++r) {
+    for (int s = r + 1; s < W; ++s)
+      if (overlap(out[r], recv_bytes[r], out[s], recv_bytes[s])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps out[%d]", r, s);
+    for (int j = 0; j < W; ++j)
+      if (overlap(out[r], recv_bytes[r], in[j], send_bytes[j])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps in[%d]", r, j);
+  }
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (W == 1) {
+    if (send_bytes[0] != recv_bytes[0])
+      return fail(B2_EINVAL, "b2_alltoall: rank 0 sends %zu bytes to itself but expects %zu", send_bytes[0], recv_bytes[0]);
+    if (recv_bytes[0]) B2_CUDA(cudaMemcpyAsync(out[0], in[0], recv_bytes[0], cudaMemcpyDeviceToDevice, s));
+    return B2_OK;
+  }
+  // A pair over the limit is seen here by its sender and its receiver.  Both still launch, with the abort flag, so that no
+  // rank waits for them and every rank's kernel sees the abort after its barrier.
+  const size_t max = b2_alltoall_max_bytes(c);
+  A2aArgs a{};
+  int rc = B2_OK;
+  for (int jj = 0; jj < W; ++jj) {
+    const int r = (me + jj) % W;
+    a.send[jj] = static_cast<const uint8_t*>(in[r]);
+    a.send_bytes[jj] = send_bytes[r];
+    a.recv[jj] = static_cast<uint8_t*>(out[r]);
+    a.recv_bytes[jj] = recv_bytes[r];
+    if (jj > 0 && rc == B2_OK && (send_bytes[r] > max || recv_bytes[r] > max))
+      rc = fail(B2_EINVAL, "b2_alltoall: rank %d sends %zu bytes to rank %d and expects %zu from it; one pair carries at most %zu "
+                "(a larger stage raises the limit: B2_STAGE_MB / stage_mb)", me, send_bytes[r], r, recv_bytes[r], max);
+  }
+  a.abort = rc != B2_OK;
+  k_alltoall<<<grid_for(c, (max + 15) / 16, 1), kThreads, 0, s>>>(c->d, a);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "all-to-all kernel launch: %s", cudaGetErrorString(e));
+  c->launches++;
+  return rc;
 }
 
 int b2_batchnorm_stats(b2_comm_t* c, float* mean, float* invstd, float count, size_t channels, float* running_mean,

@@ -92,6 +92,8 @@ SYMBOLS = [
     "b2_allreduce_op",
     "b2_allgather",
     "b2_reduce_scatter",
+    "b2_alltoall",
+    "b2_alltoall_max_bytes",
     "b2_batchnorm_stats",
     "b2_bn_forward_elemt",
     "b2_bn_backward_elemt",
@@ -184,6 +186,10 @@ def lib() -> ctypes.CDLL:
     L.b2_allgather.argtypes = [vp, vp, vp, sz, vp]
     L.b2_reduce_scatter.restype = i
     L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
+    L.b2_alltoall.restype = i
+    L.b2_alltoall.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(vp), ctypes.POINTER(sz), vp]
+    L.b2_alltoall_max_bytes.restype = sz
+    L.b2_alltoall_max_bytes.argtypes = [vp]
     L.b2_batchnorm_stats.restype = i
     L.b2_batchnorm_stats.argtypes = [vp, vp, vp, f, sz, vp, vp, ctypes.c_double, ctypes.c_double, vp, vp]
     L.b2_bn_forward_elemt.restype = i

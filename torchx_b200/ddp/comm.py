@@ -174,6 +174,11 @@ class Communicator:
     def launches(self) -> int:
         return int(N.lib().b2_comm_launch_count(self._h))
 
+    @property
+    def alltoall_max_bytes(self) -> int:
+        """The most bytes one rank may send another in one ``alltoall_`` (b2_alltoall_max_bytes)."""
+        return int(N.lib().b2_alltoall_max_bytes(self._h))
+
     # ---- collectives ---------------------------------------------------------------------------
     def allreduce_(self, t: torch.Tensor, scale: Optional[float] = None, wire: str = "bf16", algo: str = "auto",
                    stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
@@ -241,6 +246,30 @@ class Communicator:
         N.check(N.lib().b2_reduce_scatter(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()), out.numel(), dt,
                                           code, ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return out
+
+    def alltoall_(self, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor],
+                  stream: Optional[torch.cuda.Stream] = None) -> Sequence[torch.Tensor]:
+        """``outs[r]`` <- the ``ins[rank]`` of rank r, bit for bit (include/b200ddp.h: b2_alltoall).  Both are lists of world
+        contiguous tensors on this communicator's device, all of one dtype (any dtype: the copy is of bytes), of any sizes;
+        ``outs[r]`` must have as many bytes as rank r sends this rank, and one pair of ranks carries at most
+        ``alltoall_max_bytes``.  No tensor of ``outs`` may overlap another tensor of either list."""
+        if len(outs) != self.world or len(ins) != self.world:
+            raise ValueError(f"alltoall_: needs {self.world} output and {self.world} input tensors, got {len(outs)} and {len(ins)}")
+        dtypes = {t.dtype for t in (*outs, *ins)}
+        if len(dtypes) > 1:
+            raise TypeError(f"alltoall_: every tensor must have one dtype, got {sorted(str(d) for d in dtypes)}")
+        for t in (*outs, *ins):
+            self._check_tensor(t)
+
+        def ptrs(ts):
+            return (ctypes.c_void_p * self.world)(*(t.data_ptr() for t in ts))
+
+        def sizes(ts):
+            return (ctypes.c_size_t * self.world)(*(t.numel() * t.element_size() for t in ts))
+
+        N.check(N.lib().b2_alltoall(self._h, ptrs(outs), sizes(outs), ptrs(ins), sizes(ins),
+                                    ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        return outs
 
     def batchnorm_stats_(self, mean: torch.Tensor, invstd: torch.Tensor, count: float, running_mean: Optional[torch.Tensor] = None,
                          running_var: Optional[torch.Tensor] = None, *, momentum: float, eps: float,

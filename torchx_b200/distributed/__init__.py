@@ -8,7 +8,7 @@ environment contract and barrier-ordered critical sections.  Two backends behind
     otherwise) - this is what config #1 (CPU/gloo) and unmodified TorchX scripts use;
   * ``init_pg("b200")`` - the peer-buffer communicator from ``libb200ddp.so``: no TCP store, no NCCL.  ``barrier`` /
     ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor``, ``all_gather``, ``reduce_scatter_tensor``,
-    ``reduce_scatter`` and ``broadcast`` then run on that fabric.
+    ``reduce_scatter``, ``broadcast``, ``all_to_all_single`` and ``all_to_all`` then run on that fabric.
 """
 from __future__ import annotations
 
@@ -217,6 +217,47 @@ def broadcast(tensor: torch.Tensor, src: int, group: Any = None, async_op: bool 
         return dist.broadcast(tensor, src, group=group, async_op=async_op)
     _check_native_call(group, async_op)
     _COMM.broadcast_(tensor, root=src)
+    return None
+
+
+def _split_rows(t: torch.Tensor, sizes: Optional[List[int]], what: str) -> List[torch.Tensor]:
+    """``t`` cut along its first dimension into world views: ``sizes`` rows each, or evenly when ``sizes`` is None / empty."""
+    world = _COMM.world
+    if not sizes:
+        if t.size(0) % world:
+            raise ValueError(f"all_to_all_single: {what} has {t.size(0)} rows, not a multiple of the world size {world}; "
+                             f"pass {what}_split_sizes")
+        sizes = [t.size(0) // world] * world
+    sizes = [int(k) for k in sizes]
+    if len(sizes) != world or min(sizes) < 0 or sum(sizes) != t.size(0):
+        raise ValueError(f"all_to_all_single: {what}_split_sizes {sizes} must be {world} row counts >= 0 summing to the "
+                         f"{t.size(0)} rows of {what}")
+    return list(torch.split(t, sizes, dim=0))
+
+
+def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[List[int]] = None,
+                      input_split_sizes: Optional[List[int]] = None, group: Any = None, async_op: bool = False) -> Any:
+    """``torch.distributed.all_to_all_single``: ``input`` is cut along its first dimension into world blocks (evenly, or by
+    ``input_split_sizes``) and block j goes to rank j; rank r's block lands in ``output``'s r-th block (evenly, or by
+    ``output_split_sizes``).  Under ``init_pg("b200")`` the blocks are views of the two tensors, so nothing is copied
+    besides the exchange itself, and the result is the same bits; one pair of ranks carries at most
+    ``communicator().alltoall_max_bytes`` bytes."""
+    if not _on_fabric():
+        return dist.all_to_all_single(output, input, output_split_sizes=output_split_sizes, input_split_sizes=input_split_sizes,
+                                      group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.alltoall_(_split_rows(output, output_split_sizes, "output"), _split_rows(input, input_split_sizes, "input"))
+    return None
+
+
+def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[torch.Tensor], group: Any = None,
+               async_op: bool = False) -> Any:
+    """``torch.distributed.all_to_all``: ``output_tensor_list[r]`` <- rank r's ``input_tensor_list[rank]``.  Under
+    ``init_pg("b200")`` the tensors are used where they are (contiguous, one dtype), with no packing copy."""
+    if not _on_fabric():
+        return dist.all_to_all(output_tensor_list, input_tensor_list, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    _COMM.alltoall_(output_tensor_list, input_tensor_list)
     return None
 
 
