@@ -257,6 +257,20 @@ int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void*
 int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems, int dtype, int op, void* stream);
 
 /*
+ * The gradient reduce-scatter of a sharded bucket (the mini-DDP's ZeRO-1 mode), with its input gathered from a segment
+ * table as in b2_allreduce_gather:
+ *      out[i] <- round( sum_r wire( scale * segment_r(rank*block + i) ) ),   i in [0, block)
+ * The table covers the padded bucket [0, W*block) in bucket order without gaps, with the rules and error texts of
+ * b2_allreduce_gather; `mode` is any of the five B2_* gradient modes.  out[0, block) is this rank's block of what
+ * b2_allreduce_gather of the same table leaves, bit for bit, wherever that allreduce runs a rank-order kernel (every
+ * algorithm but B2_ALGO_NVLS).  An unknown mode is B2_EINVAL; block == 0 is a no-op; a poisoned communicator is
+ * B2_ESTATE.  At W == 1 the call is the local pass of b2_allreduce_gather, with its rounding.  Each rank sends and
+ * receives (W-1)/W of the wire data.
+ */
+int b2_reduce_scatter_gather(b2_comm_t* comm, void* out, size_t block, const b2_segment_t* segments, int n_segments, int mode,
+                             float scale, void* stream);
+
+/*
  * All-to-all, a bit-exact copy of bytes (any dtype): out[r] <- the recv_bytes[r] bytes rank r sends this rank, in[j] is what
  * goes to rank j (send_bytes[j] bytes).  The four arrays are HOST arrays of W entries indexed by rank, copied into the kernel
  * parameters by the call; a pointer whose count is 0 may be NULL.  No `out` range may overlap another `out` range or any

@@ -396,16 +396,16 @@ cudaError_t launch_collective(const CommDev& d, const Src& src, int kind, int gr
   }
 }
 
-// The float reduce-scatter at the communicator's world size: instantiates k_reduce_scatter<MODE, W> for W = 2 ..
-// B2_MAX_WORLD.  Only the modes whose bucket is its own wire format (B2_F32 / B2_BF16 / B2_F16) have one.
+// The float reduce-scatter at the communicator's world size: instantiates k_reduce_scatter<MODE, W> for the five gradient
+// modes and W = 2 .. B2_MAX_WORLD.
 template <int MODE, int W = 2>
-cudaError_t launch_reduce_scatter(const CommDev& d, int grid, void* out, const void* in, unsigned long long n,
+cudaError_t launch_reduce_scatter(const CommDev& d, const Src& src, int grid, void* out, const void* in, unsigned long long n,
                                   unsigned long long block, float scale, cudaStream_t s) {
-  if constexpr (W > B2_MAX_WORLD || ModeTraits<MODE>::kCastIn) {
+  if constexpr (W > B2_MAX_WORLD) {
     return cudaErrorInvalidValue;
   } else {
-    if (d.world != W) return launch_reduce_scatter<MODE, W + 1>(d, grid, out, in, n, block, scale, s);
-    k_reduce_scatter<MODE, W><<<grid, kThreads, 0, s>>>(d, out, in, n, block, scale);
+    if (d.world != W) return launch_reduce_scatter<MODE, W + 1>(d, src, grid, out, in, n, block, scale, s);
+    k_reduce_scatter<MODE, W><<<grid, kThreads, 0, s>>>(d, src, out, in, n, block, scale);
     return cudaGetLastError();
   }
 }
@@ -1089,26 +1089,69 @@ int b2_allreduce(b2_comm_t* c, void* buf, size_t n_elems, int mode, float scale,
   return allreduce_impl(c, src, buf, n_elems, mode, scale, algo, stream);
 }
 
-int b2_allreduce_gather(b2_comm_t* c, void* out, size_t n_elems, const b2_segment_t* segments, int n_segments, int mode,
-                        float scale, int algo, void* stream) {
-  if (n_elems == 0) return B2_OK;
+// The segment table of a gather call -> `src`: 1..B2_MAX_SEGMENTS entries that cover bucket elements [0, n_elems) in
+// order and without gaps, each with a source pointer.  `fn` names the call in the error texts.
+static int segment_table(const char* fn, const b2_segment_t* segments, int n_segments, size_t n_elems, Src& src) {
   if (!segments || n_segments <= 0 || n_segments > B2_MAX_SEGMENTS)
-    return fail(B2_EINVAL, "b2_allreduce_gather: need 1..%d segments (got %d)", B2_MAX_SEGMENTS, n_segments);
-  Src src;
+    return fail(B2_EINVAL, "%s: need 1..%d segments (got %d)", fn, B2_MAX_SEGMENTS, n_segments);
   src.nseg = n_segments;
   src.off = 0;
   unsigned long long at = 0;
   for (int i = 0; i < n_segments; ++i) {
     if (segments[i].begin != at || segments[i].end <= at || !segments[i].src)
-      return fail(B2_EINVAL, "b2_allreduce_gather: segment %d does not continue the bucket at element %llu", i, at);
+      return fail(B2_EINVAL, "%s: segment %d does not continue the bucket at element %llu", fn, i, at);
     src.ptr[i] = segments[i].src;
     src.begin[i] = at;
     at = segments[i].end;
   }
-  if (at != n_elems) return fail(B2_EINVAL, "b2_allreduce_gather: segments cover %llu elements, bucket has %zu", at, n_elems);
+  if (at != n_elems) return fail(B2_EINVAL, "%s: segments cover %llu elements, bucket has %zu", fn, at, n_elems);
   for (int i = n_segments; i <= B2_MAX_SEGMENTS; ++i) src.begin[i] = at;
   for (int i = n_segments; i < B2_MAX_SEGMENTS; ++i) src.ptr[i] = nullptr;
+  return B2_OK;
+}
+
+int b2_allreduce_gather(b2_comm_t* c, void* out, size_t n_elems, const b2_segment_t* segments, int n_segments, int mode,
+                        float scale, int algo, void* stream) {
+  if (n_elems == 0) return B2_OK;
+  Src src;
+  if (const int rc = segment_table("b2_allreduce_gather", segments, n_segments, n_elems, src)) return rc;
   return allreduce_impl(c, src, out, n_elems, mode, scale, algo, stream);
+}
+
+int b2_reduce_scatter_gather(b2_comm_t* c, void* out, size_t block, const b2_segment_t* segments, int n_segments, int mode,
+                             float scale, void* stream) {
+  if (!known_mode(mode)) return fail(B2_EINVAL, "b2_reduce_scatter_gather: unknown mode %d", mode);
+  if (block == 0) return B2_OK;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!out) return fail(B2_EINVAL, "b2_reduce_scatter_gather: null buffer");
+  const int W = c->d.world;
+  Src src;
+  if (const int rc = segment_table("b2_reduce_scatter_gather", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
+  if (const int rc = check_not_poisoned(c)) return rc;
+  if (W == 1) {  // the local pass of b2_allreduce_gather, rounding included
+    const int rc = local_pass_impl(src, out, block, mode, scale, c->device, stream);
+    if (rc == B2_OK) c->launches++;
+    return rc;
+  }
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t eb = elem_bytes(mode);
+  const size_t cap = c->d.slice_cap / wire_vec_bytes(mode) * 8;  // elements of a block one recv region holds (whole vecs)
+  uint8_t* po = static_cast<uint8_t*>(out);
+  size_t off = 0;
+  while (off < block) {
+    const size_t n = block - off < cap ? block - off : cap;
+    const int grid = grid_for(c, (n + 7) / 8, vecs_per_trip(W));
+    src.off = off;  // every block's launch-local element 0 is bucket element j * block + off
+    cudaError_t e = cudaErrorInvalidValue;  // never guess a mode
+    with_mode(mode, [&](auto m) {
+      e = launch_reduce_scatter<decltype(m)::value>(c->d, src, grid, po + off * eb, nullptr, n, block, scale, s);
+    });
+    if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
+    c->launches++;
+    off += n;
+  }
+  return B2_OK;
 }
 
 int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) {
@@ -1309,7 +1352,7 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
     if (sum) {
       const int grid = grid_for(c, (n + 7) / 8, vecs_per_trip(W));
       with_mode(mode, [&](auto m) {
-        e = launch_reduce_scatter<decltype(m)::value>(c->d, grid, po + off * eb, pi + off * eb, n, n_elems, scale, s);
+        e = launch_reduce_scatter<decltype(m)::value>(c->d, kNoSrc, grid, po + off * eb, pi + off * eb, n, n_elems, scale, s);
       });
     } else {
       const int grid = grid_for(c, (n * eb + 15) / 16, 1);

@@ -10,6 +10,10 @@
 // vec, so every block has its own alignment flag and the element fallbacks of the local accesses handle the rest.  The
 // thread that reads vec v of my own block in phase A is the one that writes vec v of `out` in phase B, so `out` may be my
 // block of `in` (the in-place form).  The op counter, stage parity and flag sequence are those of every other collective.
+//
+// The float kernel also reads its input through a segment table (b2_reduce_scatter_gather: the sharded bucket of the
+// mini-DDP, zero-copy as b2_allreduce_gather).  `src.nseg == 0` is the flat `in` above; otherwise element i of block j of
+// this launch is bucket element j * block + src.off + i, and `in` is not read.
 #pragma once
 
 #include "b2_dev.cuh"
@@ -17,8 +21,9 @@
 
 // Float SUM / AVG: out <- round(sum_r wire(scale * in_r[rank block])), the rank-order fp32 sum of k_twoshot.
 template <int MODE, int W>
-__global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter(CommDev c, void* out, const void* in, unsigned long long n,
-                                                                 unsigned long long block, float scale) {
+__global__ void __launch_bounds__(kThreads, 1)
+    k_reduce_scatter(CommDev c, const __grid_constant__ Src src, void* out, const void* in, unsigned long long n,
+                     unsigned long long block, float scale) {
   using namespace dev;
   using Elem = typename ModeTraits<MODE>::Elem;
   constexpr int WVB = Wire<MODE>::kBytes;
@@ -38,8 +43,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter(CommDev c, void*
       const unsigned long long v = v0 + u * stride;
 #pragma unroll
       for (int jj = 0; jj < W; ++jj) {
-        const Elem* src = static_cast<const Elem*>(in) + slice_of<W>(c.rank, jj) * block;
-        if (v < V) x[u][jj] = load_in<MODE>(src, v * 8, n, buf_aligned<MODE>(src));
+        // element v * 8 of block j, addressed from the start of `in` / of this launch's part of the bucket
+        const unsigned long long jb = slice_of<W>(c.rank, jj) * block;
+        if (v < V) x[u][jj] = load_src<MODE>(src, in, jb + v * 8, jb + n, buf_aligned<MODE>(static_cast<const Elem*>(in) + jb));
       }
     }
 #pragma unroll

@@ -92,6 +92,7 @@ SYMBOLS = [
     "b2_allreduce_op",
     "b2_allgather",
     "b2_reduce_scatter",
+    "b2_reduce_scatter_gather",
     "b2_alltoall",
     "b2_alltoall_max_bytes",
     "b2_batchnorm_stats",
@@ -186,6 +187,8 @@ def lib() -> ctypes.CDLL:
     L.b2_allgather.argtypes = [vp, vp, vp, sz, vp]
     L.b2_reduce_scatter.restype = i
     L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
+    L.b2_reduce_scatter_gather.restype = i
+    L.b2_reduce_scatter_gather.argtypes = [vp, vp, sz, ctypes.POINTER(B2Segment), i, i, f, vp]
     L.b2_alltoall.restype = i
     L.b2_alltoall.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(vp), ctypes.POINTER(sz), vp]
     L.b2_alltoall_max_bytes.restype = sz

@@ -247,6 +247,20 @@ class Communicator:
                                           code, ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return out
 
+    def reduce_scatter_gather_(self, out: torch.Tensor, segments, n_segments: int, scale: Optional[float] = None,
+                               wire: str = "bf16", stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+        """``out`` (``block`` elements) <- block ``rank`` of ``allreduce_gather_`` over the padded bucket of ``world * block``
+        elements the segment table covers (include/b200ddp.h: b2_reduce_scatter_gather): the same bits that allreduce leaves
+        there wherever it sums in rank order, moving only (W-1)/W of the wire data.  The gradient shard of the sharded
+        mini-DDP."""
+        self._check_tensor(out)
+        if scale is None:
+            scale = 1.0 / self.world
+        N.check(N.lib().b2_reduce_scatter_gather(self._h, ctypes.c_void_p(out.data_ptr()), out.numel(), segments, n_segments,
+                                                 mode_for(out, wire), ctypes.c_float(scale),
+                                                 ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        return out
+
     def alltoall_(self, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor],
                   stream: Optional[torch.cuda.Stream] = None) -> Sequence[torch.Tensor]:
         """``outs[r]`` <- the ``ins[rank]`` of rank r, bit for bit (include/b200ddp.h: b2_alltoall).  Both are lists of world

@@ -49,7 +49,8 @@ class _Bucket:
     def __init__(self, spec: BucketSpec, params: List[nn.Parameter], device: torch.device) -> None:
         self.spec = spec
         self.params = params
-        self.flat = torch.zeros(spec.numel, dtype=params[0].dtype, device=device)
+        self.dtype = params[0].dtype
+        self.flat = torch.zeros(spec.numel, dtype=self.dtype, device=device)
         # like the Reducer, give each view the parameter's own (dense) strides so a channels_last weight gets a
         # channels_last gradient view and the bucket's element order is the gradient's memory order
         self.views = [_view_like(self.flat[o : o + n], p) for o, n, p in zip(spec.offsets, spec.numels, params)]
@@ -68,6 +69,39 @@ class _Bucket:
             for i, (o, n) in enumerate(zip(spec.offsets, spec.numels)):
                 self.segments[i].begin = o
                 self.segments[i].end = o + n
+        self.block = 0  # sharded mode (ZeroRedundancyOptimizer): elements of this rank's shard, else 0
+
+    def shard(self, world: int, device: torch.device) -> None:
+        """Switch to the ZeRO-1 layout: the bucket is padded to world * block elements, the parameters move into one
+        persistent flat buffer of that size, and the full-size gradient bucket gives way to this rank's block-sized
+        gradient shard.  The pad reads as zero through a last segment that points at a small zero tensor."""
+        from .zero import padded_block
+
+        n_el = self.spec.numel
+        self.block = padded_block(n_el, world)
+        pad = world * self.block - n_el
+        self.flat, self.views = None, None  # the reduced gradient exists only as the shard
+        self.param_flat = torch.zeros(world * self.block, dtype=self.dtype, device=device)
+        with torch.no_grad():
+            for o, n, p in zip(self.spec.offsets, self.spec.numels, self.params):
+                v = _view_like(self.param_flat[o : o + n], p)  # the parameter's own strides: channels_last stays so
+                v.copy_(p.data)
+                p.data = v
+        self.shard_grad = torch.zeros(self.block, dtype=self.dtype, device=device)
+        self.pad_zeros = torch.zeros(max(pad, 1), dtype=self.dtype, device=device)
+
+        def table(ranges):
+            segs = (N.B2Segment * (len(ranges) + (pad > 0)))()
+            for i, (o, n) in enumerate(ranges):
+                segs[i].begin, segs[i].end = o, o + n
+            if pad:
+                segs[-1].src, segs[-1].begin, segs[-1].end = self.pad_zeros.data_ptr(), n_el, n_el + pad
+            return segs
+
+        P = len(self.params)
+        self.segments = table(list(zip(self.spec.offsets, self.spec.numels))) if P + (pad > 0) <= N.B2_MAX_SEGMENTS else None
+        self.copy_segments = table([(0, n_el)])  # the fallback: the gradients copied into one scratch tensor
+        self.scratch = None
 
 
 class DistributedDataParallel(nn.Module):
@@ -124,6 +158,10 @@ class DistributedDataParallel(nn.Module):
         self._profile: Optional[list] = None
         self.copied_in_buckets = 0   # buckets that needed the multi-tensor copy-in (zero-copy not applicable), for tests / bench
         self.gathered_buckets = 0    # buckets whose gradients were read in place by the kernel
+        self.sharded = False         # ZeRO-1 layout (ZeroRedundancyOptimizer): each rank keeps one block of every bucket
+        self._shard_grads: List = []  # (optimizer view, its gradient shard view): attached after every synced backward
+        self._shard_grads_live = False  # the shards hold a reduced gradient that zero_grad() has not cleared
+        self._synced_backwards = 0
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad_ready) for p in self._params]
         # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen
         from torchx_b200.nn.bn2d import convert_batchnorm
@@ -165,6 +203,16 @@ class DistributedDataParallel(nn.Module):
             bufs = [b.data for b in self.module.buffers()]
             if bufs:
                 self._broadcast_coalesced(bufs)
+
+    def _enable_sharding(self) -> None:
+        """The ZeRO-1 layout of every bucket (_Bucket.shard); ZeroRedundancyOptimizer's constructor calls it."""
+        if self.sharded:
+            raise RuntimeError("this DistributedDataParallel is already sharded by a ZeroRedundancyOptimizer")
+        if self._synced_backwards:
+            raise RuntimeError("ZeroRedundancyOptimizer must be constructed before the model's first backward")
+        for b in self.buckets:
+            b.shard(self.world_size, self.device)
+        self.sharded = True
 
     # ---- training step -----------------------------------------------------------------------------
     def _reset_reducer_state(self) -> None:
@@ -210,7 +258,7 @@ class DistributedDataParallel(nn.Module):
     def _gatherable(self, b: _Bucket, grads: List[torch.Tensor]) -> bool:
         """The kernel can read a gradient in place when its memory order IS the bucket's element order: same dtype,
         same (dense) strides as the bucket view the parameter's layout produced."""
-        dt = b.flat.dtype
+        dt = b.dtype
         for g, st in zip(grads, b.view_strides):
             if g.dtype != dt or not g.is_cuda or tuple(s_ for s_, z in zip(g.stride(), g.shape) if z != 1) != st:
                 return False
@@ -224,6 +272,9 @@ class DistributedDataParallel(nn.Module):
                 raise RuntimeError("a parameter finished backward without a gradient (unused parameters are not supported)")
             grads.append(g)
         gather = self.zero_copy and b.segments is not None and self._gatherable(b, grads)
+        if self.sharded:
+            self._launch_shard(b, grads, gather)
+            return
         if not gather:
             src, dst = [], []
             for g, v in zip(grads, b.views):
@@ -257,6 +308,45 @@ class DistributedDataParallel(nn.Module):
             self._profile.append((t0, t1, b.spec.numel * 2 * b.flat.element_size()))
         b.launched = True
 
+    def _launch_shard(self, b: _Bucket, grads: List[torch.Tensor], gather: bool) -> None:
+        """Sharded mode: reduce-scatter the bucket (padded to W blocks) into this rank's gradient shard, with the wire,
+        scale, order and stream of the allreduce.  Its gradients are read in place, or copied into one scratch tensor
+        first when they cannot be (more segments than a table holds, another layout, zero_copy=False)."""
+        if self._next_bucket == 0 and self._shard_grads_live:
+            # Unsharded, this backward would add into the reduced gradients still in p.grad.  The sharded gradients live
+            # only in the shards, which this backward overwrites: refuse rather than drop the earlier micro-batch.  (Raised
+            # before any bucket of this backward is launched, on every rank alike.)
+            raise RuntimeError(
+                "a second synced backward before zero_grad(): the sharded mini-DDP does not accumulate reduced gradients "
+                "across synced backwards; call zero_grad() after step(), and accumulate micro-batches under no_sync()")
+        if gather:
+            segs = b.segments
+            for seg, g in zip(segs, grads):
+                seg.src = g.data_ptr()
+            self.gathered_buckets += 1
+        else:
+            b.scratch = torch.empty(b.spec.numel, dtype=b.dtype, device=self.device)
+            views = [_view_like(b.scratch[o : o + n], p) for o, n, p in zip(b.spec.offsets, b.spec.numels, b.params)]
+            torch._foreach_copy_(views, grads)
+            segs = b.copy_segments
+            segs[0].src = b.scratch.data_ptr()
+            self.copied_in_buckets += 1
+        cur = torch.cuda.current_stream(self.device)
+        self._ready_event.record(cur)
+        self._comm_stream.wait_event(self._ready_event)
+        if self._profile is not None:
+            t0 = torch.cuda.Event(enable_timing=True)
+            t0.record(self._comm_stream)
+        # the gradients (and the scratch copy) stay referenced until _finalize_backward has made the compute stream wait
+        self.comm.reduce_scatter_gather_(b.shard_grad, segs, len(segs), scale=1.0 / self.world_size, wire=self.wire,
+                                         stream=self._comm_stream)
+        b.done.record(self._comm_stream)
+        if self._profile is not None:
+            t1 = torch.cuda.Event(enable_timing=True)
+            t1.record(self._comm_stream)
+            self._profile.append((t0, t1, 2 * b.spec.nbytes))
+        b.launched = True
+
     def _finalize_backward(self) -> None:
         self._callback_queued = False
         try:
@@ -268,8 +358,17 @@ class DistributedDataParallel(nn.Module):
             cur = torch.cuda.current_stream(self.device)
             for b in self.buckets:
                 cur.wait_event(b.done)
-                for p, v in zip(b.params, b.views):
-                    p.grad = v  # gradient_as_bucket_view: the optimizer reads the averaged bucket in place
+                if self.sharded:
+                    b.scratch = None
+                    for p in b.params:
+                        p.grad = None  # frees the full-size gradients: the reduced ones exist only as the shards
+                else:
+                    for p, v in zip(b.params, b.views):
+                        p.grad = v  # gradient_as_bucket_view: the optimizer reads the averaged bucket in place
+            for v, g in self._shard_grads:
+                v.grad = g
+            self._shard_grads_live = bool(self._shard_grads)
+            self._synced_backwards += 1
             self.comm.check()
         finally:
             self._next_bucket = 0

@@ -1,0 +1,309 @@
+"""ZeRO stage 1 for the mini-DDP: each rank keeps the optimizer state of one block of every bucket (DESIGN.md 2.5).
+
+torch's ``ZeroRedundancyOptimizer`` needs a ``torch.distributed`` process group; under ``init_pg("b200")`` there is none.
+This one runs on the native communicator instead:
+
+  * the backward reduce-scatters every bucket into this rank's gradient shard (``b2_reduce_scatter_gather``: the bits the
+    unsharded bucket allreduce leaves in that block, read zero-copy from the per-parameter gradients);
+  * ``step()`` steps the inner optimizer on this rank's slice of the parameters only, then all-gathers every bucket's
+    flat parameter buffer in place (exact bytes).
+
+SGD, Adam and AdamW are elementwise, so stepping a slice gives the bits of stepping the whole tensor: the parameters
+stay bit-equal to those of the unsharded mini-DDP under the same optimizer, and the consolidated state to its state.
+"""
+from __future__ import annotations
+
+from typing import Any, Dict, List, Optional, Sequence, Tuple
+
+import torch
+
+from .ddp import DistributedDataParallel, _view_like
+
+# the elementwise optimizers: a slice of a tensor steps to the bits of the same slice of the stepped tensor
+SUPPORTED = (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW)
+
+
+def padded_block(numel: int, world: int) -> int:
+    """Elements of one rank's block of a bucket of ``numel`` elements: ceil(numel / world) rounded up to a whole vec
+    (8 elements), so every block starts on a vec.  The bucket is padded to world * block elements."""
+    return (-(-numel // world) + 7) // 8 * 8
+
+
+def block_intersections(offsets: Sequence[int], numels: Sequence[int], block: int, rank: int) -> List[Tuple[int, int, int]]:
+    """(index, lo, hi) for each parameter whose bucket range [offset, offset + numel) meets rank's block
+    [rank * block, (rank + 1) * block): bucket elements [lo, hi) of parameter ``index`` belong to this rank."""
+    b0, b1 = rank * block, (rank + 1) * block
+    out = []
+    for i, (o, n) in enumerate(zip(offsets, numels)):
+        lo, hi = max(o, b0), min(o + n, b1)
+        if lo < hi:
+            out.append((i, lo, hi))
+    return out
+
+
+def _ordered(comm: Any, launch) -> None:
+    from torchx_b200.nn.batchnorm import _ordered as ordered
+
+    ordered(comm, launch)
+
+
+class ZeroRedundancyOptimizer(torch.optim.Optimizer):
+    """``optimizer_class`` (SGD, Adam or AdamW, with any of their options) over this rank's shard of a mini-DDP's
+    parameters.  Constructing it switches ``model`` into sharded mode, which must happen before its first backward.
+
+    ``params`` defaults to every trainable parameter of the model; torch-style groups over those parameters are accepted,
+    and every trainable parameter must be in exactly one group.  ``param_groups`` are the inner optimizer's groups, so
+    ``torch.optim.lr_scheduler`` works.
+
+    After a synced backward the model parameters' ``.grad`` are None (the reduced gradients exist only as the shards), so
+    clip with ``clip_grad_norm_`` of this class: ``torch.nn.utils.clip_grad_norm_(model.parameters(), ...)`` sees no
+    gradients and clips nothing."""
+
+    _step_supports_amp_scaling = True  # GradScaler hands itself to step(): the found-inf decision is made rank-global there
+
+    def __init__(self, model: DistributedDataParallel, optimizer_class: type, params: Optional[Any] = None, **defaults: Any) -> None:
+        if optimizer_class not in SUPPORTED:
+            raise TypeError(f"ZeroRedundancyOptimizer supports {', '.join(c.__name__ for c in SUPPORTED)}, "
+                            f"not {getattr(optimizer_class, '__name__', optimizer_class)}")
+        if not isinstance(model, DistributedDataParallel):
+            raise TypeError("ZeroRedundancyOptimizer shards a torchx_b200.ddp.DistributedDataParallel")
+        groups = _normalize_groups(model._params if params is None else params)
+        _check_groups(groups, model._params)
+        super().__init__(groups, defaults)  # validates the groups and fills in the defaults
+        self.model = model
+        self.comm = model.comm
+        self.optimizer_class = optimizer_class
+        self._full_groups = [list(g["params"]) for g in self.param_groups]  # model parameters, the user's order
+        model._enable_sharding()
+
+        W, r = model.world_size, self.comm.rank
+        where: Dict[int, Tuple[Any, int, int]] = {}  # id(param) -> (bucket, offset, numel)
+        for b in model.buckets:
+            for p, o, n in zip(b.params, b.spec.offsets, b.spec.numels):
+                where[id(p)] = (b, o, n)
+        self._where = where
+        # views[id(param)] = (view of the flat parameter buffer, bucket elements lo, hi): this rank's slice of it
+        self._views: Dict[int, Tuple[torch.Tensor, int, int]] = {}
+        for b in model.buckets:
+            for i, lo, hi in block_intersections(b.spec.offsets, b.spec.numels, b.block, r):
+                v = b.param_flat[lo:hi]
+                self._views[id(b.params[i])] = (v, lo, hi)
+                model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block]))
+        inner_groups = []
+        for g, ps in zip(self.param_groups, self._full_groups):
+            inner = {k: val for k, val in g.items() if k != "params"}
+            inner["params"] = [self._views[id(p)][0] for p in ps if id(p) in self._views]
+            inner_groups.append(inner)
+        self.optim = optimizer_class(inner_groups, **defaults)
+        self.param_groups = self.optim.param_groups  # scheduler writes reach the inner optimizer
+        self.state = self.optim.state
+        self.defaults = self.optim.defaults
+        self._world, self._rank = W, r
+        self._stepped = False  # the same on every rank: the skip decision under a GradScaler is rank-global
+
+    # ---- step ------------------------------------------------------------------------------------
+    @torch.no_grad()
+    def step(self, closure=None, grad_scaler=None):  # noqa: D401
+        """Inner step on this rank's shard, then an in-place all-gather of every bucket's parameter buffer.  Under a
+        GradScaler the found-inf flags are first reduced with MAX over the ranks, in the very tensors ``update()`` reads,
+        so an inf in one rank's shard makes every rank skip the step and back off its scale alike.
+
+        This relies on GradScaler passing itself as ``grad_scaler`` (torch 2.11 warns that the keyword is deprecated).  Its
+        replacement hands the optimizer only a sum of the found-inf tensors, a new tensor, while ``update()`` reads the
+        per-device ones: a MAX reduced into that sum would not reach the scale update, and the ranks' scales would drift
+        apart.  Should torch drop the keyword, ``step()`` stops being called with it and a GradScaler run raises below."""
+        if closure is not None:
+            raise RuntimeError("ZeroRedundancyOptimizer.step does not take a closure")
+        if grad_scaler is None and getattr(self, "found_inf", None) is not None:
+            raise RuntimeError("this GradScaler no longer passes itself to step(): the rank-global inf check cannot run")
+        if grad_scaler is not None:
+            from torch.amp.grad_scaler import OptState
+
+            st = grad_scaler._per_optimizer_states[id(self)]
+            if st["stage"] is OptState.READY:
+                grad_scaler.unscale_(self)
+            found = st["found_inf_per_device"]
+            if not found:  # this rank holds no gradient: it still takes part in the reduction
+                found[self.model.device] = torch.zeros((), dtype=torch.float32, device=self.model.device)
+            for t in found.values():
+                _ordered(self.comm, lambda s, t=t: self.comm.allreduce_op_(t, "max", stream=s))
+            if sum(t.item() for t in found.values()):
+                return None
+        self.optim.step()
+        self._stepped = True
+        for b in self.model.buckets:
+            own = b.param_flat[self._rank * b.block : (self._rank + 1) * b.block]
+            _ordered(self.comm, lambda s, b=b, own=own: self.comm.allgather_(b.param_flat, own, stream=s))
+        return None
+
+    def zero_grad(self, set_to_none: bool = True) -> None:
+        """Clears the gradient shards and the model parameters' ``.grad``.  Required between a step and the next synced
+        backward: the reduced gradients live only in the shards, which a synced backward overwrites (it raises instead)."""
+        self.model._shard_grads_live = False
+        for v, g in self.model._shard_grads:
+            if set_to_none:
+                v.grad = None
+            else:
+                g.zero_()
+                v.grad = g
+        for p in self.model._params:
+            if set_to_none:
+                p.grad = None
+            elif p.grad is not None:
+                p.grad.detach_().zero_()
+
+    @torch.no_grad()
+    def clip_grad_norm_(self, max_norm: float) -> torch.Tensor:
+        """Clips the sharded gradients in place by their global 2-norm and returns that norm (fp32, the same bits on
+        every rank): the sqrt of the rank-order fp32 sum of each rank's fp32 sum of squares over its shard.  The clip
+        coefficient is torch's, ``max_norm / (norm + 1e-6)`` clamped to 1."""
+        dev = self.model.device
+        grads = [v.grad for v, _ in self.model._shard_grads if v.grad is not None]
+        sq = torch.zeros(1, dtype=torch.float32, device=dev)
+        if grads:
+            sq = torch.stack([g.float().square().sum() for g in grads]).sum().reshape(1)
+        _ordered(self.comm, lambda s: self.comm.allreduce_op_(sq, "sum", stream=s))
+        norm = sq.sqrt()[0]
+        coef = torch.clamp(max_norm / (norm + 1e-6), max=1.0)
+        if grads:
+            torch._foreach_mul_(grads, coef.to(grads[0].dtype))
+        return norm
+
+    # ---- checkpoints -----------------------------------------------------------------------------
+    def _index(self) -> List[torch.nn.Parameter]:
+        return [p for ps in self._full_groups for p in ps]  # the unsharded optimizer's param index order
+
+    def _keys(self, group: Dict[str, Any]) -> List[str]:
+        """Per-parameter state keys of a group once it has stepped, in the order the optimizer class creates them."""
+        if self.optimizer_class is torch.optim.SGD:
+            return ["momentum_buffer"] if group["momentum"] != 0 else []
+        return ["step", "exp_avg", "exp_avg_sq"] + (["max_exp_avg_sq"] if group["amsgrad"] else [])
+
+    def consolidate_state_dict(self, to: int = 0) -> None:
+        """Collective: all-gathers every rank's state slices (exact bytes) so that ``state_dict()`` on rank ``to``
+        returns the state dict the unsharded optimizer would have, in host memory (as torch's ZeroRedundancyOptimizer
+        keeps it).  On the GPU only one bucket of one state at a time is ever full-size; the other ranks keep nothing."""
+        self._consolidated = None  # an earlier checkpoint's copy is not held alongside this one
+        params = self._index()
+        r, W, dev = self._rank, self._world, self.model.device
+        keys_of = {id(p): self._keys(g) if self._stepped else [] for g, ps in zip(self.param_groups, self._full_groups) for p in ps}
+        tensor_keys = [k for k in ("exp_avg", "exp_avg_sq", "max_exp_avg_sq", "momentum_buffer")
+                       if any(k in ks for ks in keys_of.values())]
+        # Adam's scalar `step`: one fp32 per parameter from every rank, taken from the lowest rank that holds a slice.  Read
+        # before any collective is issued, so that no host sync waits behind them.
+        n = len(params)
+        own_steps = torch.zeros(n, dtype=torch.float32, device=dev)
+        for i, p in enumerate(params):
+            st = self.optim.state.get(self._views[id(p)][0], {}).get("step") if id(p) in self._views else None
+            if st is not None:
+                own_steps[i : i + 1].copy_(st.reshape(1), non_blocking=True)
+        steps = torch.zeros(W * n, dtype=torch.float32, device=dev)
+        steps[r * n : (r + 1) * n].copy_(own_steps)
+        full: Dict[str, Dict[int, torch.Tensor]] = {k: {} for k in tensor_keys}
+        for k in tensor_keys:
+            for b in self.model.buckets:
+                buf = torch.zeros(W * b.block, dtype=b.dtype, device=dev)
+                for p in b.params:
+                    if id(p) in self._views:
+                        v, lo, hi = self._views[id(p)]
+                        st = self.optim.state.get(v, {}).get(k)
+                        if st is not None:
+                            buf[lo:hi].copy_(st)
+                own = buf[r * b.block : (r + 1) * b.block]
+                _ordered(self.comm, lambda s, buf=buf, own=own: self.comm.allgather_(buf, own, stream=s))
+                if r == to:
+                    host = buf.cpu()
+                    for p, o, numel in zip(b.params, b.spec.offsets, b.spec.numels):
+                        full[k][id(p)] = _view_like(host[o : o + numel], p).clone()
+                del buf, own
+        _ordered(self.comm, lambda s: self.comm.allgather_(steps, steps[r * n : (r + 1) * n], stream=s))
+        if r != to:
+            return
+        steps_h = steps.view(W, n).cpu()
+        state: Dict[int, Dict[str, Any]] = {}
+        for i, p in enumerate(params):
+            entry: Dict[str, Any] = {}
+            for k in keys_of[id(p)]:
+                if k == "step":
+                    owner = next(q for q in range(W) if _owns(self._where[id(p)], q))
+                    entry[k] = steps_h[owner, i].clone()
+                else:
+                    entry[k] = full[k][id(p)]
+            if entry:
+                state[i] = entry
+        groups, at = [], 0
+        for g, ps in zip(self.param_groups, self._full_groups):
+            d = {k: val for k, val in g.items() if k != "params"}
+            d["params"] = list(range(at, at + len(ps)))
+            at += len(ps)
+            groups.append(d)
+        self._consolidated = {"state": state, "param_groups": groups}
+
+    def state_dict(self) -> Dict[str, Any]:
+        """After ``consolidate_state_dict(to)``, on rank ``to``: the state dict of the unsharded optimizer (its
+        param_groups and param indices; full-size per-parameter state)."""
+        sd = getattr(self, "_consolidated", None)
+        if sd is None:
+            raise RuntimeError("call consolidate_state_dict(to) on every rank first; state_dict() returns on rank `to` only")
+        return sd
+
+    def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
+        """Loads the full (unsharded) form on every rank, keeping this rank's slices."""
+        groups = state_dict["param_groups"]
+        if len(groups) != len(self._full_groups) or any(len(g["params"]) != len(ps) for g, ps in zip(groups, self._full_groups)):
+            raise ValueError("the state dict's param groups do not match this optimizer's")
+        inner_state: Dict[int, Dict[str, Any]] = {}
+        inner_groups, at = [], 0
+        for g, ps in zip(groups, self._full_groups):
+            d = {k: val for k, val in g.items() if k != "params"}
+            d["params"] = []
+            for idx, p in zip(g["params"], ps):
+                if id(p) not in self._views:
+                    continue
+                v, lo, hi = self._views[id(p)]
+                o = self._where[id(p)][1]
+                entry = {}
+                for k, val in state_dict["state"].get(idx, {}).items():
+                    if k != "step" and torch.is_tensor(val):  # per-element state (a 0-dim parameter's too): this rank's slice
+                        mem = _view_like(torch.empty(p.numel(), dtype=val.dtype, device=p.device), p)
+                        mem.copy_(val)  # the parameter's memory order, as the flat buffer holds it
+                        val = mem.as_strided((p.numel(),), (1,))[lo - o : hi - o]
+                    entry[k] = val.clone() if torch.is_tensor(val) else val  # never alias the caller's state
+                if entry:
+                    inner_state[at] = entry
+                d["params"].append(at)
+                at += 1
+            inner_groups.append(d)
+        self.optim.load_state_dict({"state": inner_state, "param_groups": inner_groups})
+        self._stepped = bool(state_dict["state"])
+        self.param_groups = self.optim.param_groups
+        self.state = self.optim.state
+
+
+def _owns(where, rank: int) -> bool:
+    b, o, n = where
+    return max(o, rank * b.block) < min(o + n, (rank + 1) * b.block)
+
+
+def _normalize_groups(params: Any) -> List[Dict[str, Any]]:
+    params = list(params)
+    if not params:
+        raise ValueError("ZeroRedundancyOptimizer got an empty parameter list")
+    if not isinstance(params[0], dict):
+        params = [{"params": params}]
+    return [dict(g, params=list(g["params"])) for g in params]
+
+
+def _check_groups(groups: List[Dict[str, Any]], trainable: Sequence[torch.nn.Parameter]) -> None:
+    """Every trainable parameter of the model in exactly one group, and nothing else."""
+    want = {id(p) for p in trainable}
+    seen = set()
+    for g in groups:
+        for p in g["params"]:
+            if id(p) not in want:
+                raise ValueError("a parameter group holds a tensor that is not a trainable parameter of the model")
+            if id(p) in seen:
+                raise ValueError("a parameter appears in more than one group (or twice in one)")
+            seen.add(id(p))
+    if seen != want:
+        raise ValueError(f"{len(want - seen)} trainable parameters of the model are in no parameter group")
