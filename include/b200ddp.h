@@ -47,7 +47,7 @@ extern "C" {
 #endif
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
-                            b2_reduce_scatter, b2_bn_*_elemt and b2_alltoall*, which only add symbols: a binding that needs them
+                            b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall* and b2_reduce_scatter_step, which only add symbols: a binding that needs them
                             fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -269,6 +269,62 @@ int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems
  */
 int b2_reduce_scatter_gather(b2_comm_t* comm, void* out, size_t block, const b2_segment_t* segments, int n_segments, int mode,
                              float scale, void* stream);
+
+/*
+ * The same reduce-scatter with the optimizer step fused into it (the ZeRO-1 mini-DDP's overlap_with_ddp mode): instead of
+ * storing this rank's reduced block, the kernel steps this rank's block of the flat fp32 parameter buffer and its optimizer
+ * state with it, element by element, with the arithmetic of torch's fused optimizers (torch._fused_sgd_, _fused_adam_,
+ * _fused_adamw_; fp32 parameters, no grad scale, no amsgrad):
+ *      g[i] = round( sum_r wire( scale * segment_r(rank*block + i) ) )   (what b2_reduce_scatter_gather stores)
+ *      param[i], state[i] <- step(group of i, param[i], g[i], state[i]),  i in [0, block)
+ * `opt->param`, `opt->state0` and `opt->state1` point at `block` fp32 elements each: this rank's block of the parameter
+ * buffer, then momentum_buffer (SGD) or exp_avg and exp_avg_sq (Adam / AdamW).  The runs of `opt` assign block elements to
+ * parameter groups: run k covers block elements [run_begin[k], run_begin[k+1]) (run_begin[0] == 0, increasing,
+ * run_begin[n_runs] == block), and an element of a run whose group is B2_OPT_NO_GROUP (the pad) is not touched.
+ * Modes B2_F32_WIRE_BF16, B2_F32 and B2_F32_WIRE_F16 only.  B2_EINVAL, before anything is launched, for: the checks of
+ * b2_reduce_scatter_gather, another mode, an unknown kind, a null `opt` or parameter pointer, a null state pointer the kind
+ * reads, 0 or more than B2_OPT_MAX_GROUPS groups, 0 or more than B2_OPT_MAX_RUNS runs, runs that do not tile the block, a
+ * group index out of range, or block >= 2^32.
+ */
+#define B2_OPT_SGD 1
+#define B2_OPT_ADAM 2
+#define B2_OPT_ADAMW 3
+#define B2_OPT_MAX_GROUPS 8
+#define B2_OPT_MAX_RUNS 128
+#define B2_OPT_NO_GROUP 255
+typedef struct b2_optim_group {
+  double lr;
+  double weight_decay;
+  double momentum;  /* SGD */
+  double dampening; /* SGD */
+  double beta1;     /* Adam / AdamW */
+  double beta2;     /* Adam / AdamW */
+  double eps;       /* Adam / AdamW */
+  int nesterov;     /* SGD */
+  int maximize;
+} b2_optim_group_t;
+
+typedef struct b2_optim {
+  int kind;     /* B2_OPT_* */
+  int n_groups; /* 1..B2_OPT_MAX_GROUPS */
+  int n_runs;   /* 1..B2_OPT_MAX_RUNS */
+  float* param;
+  float* state0; /* SGD: momentum_buffer (may be NULL when every group's momentum is 0); Adam / AdamW: exp_avg */
+  float* state1; /* Adam / AdamW: exp_avg_sq; SGD: unused */
+  uint64_t run_begin[B2_OPT_MAX_RUNS + 1];
+  uint8_t run_group[B2_OPT_MAX_RUNS];
+  float run_step[B2_OPT_MAX_RUNS]; /* Adam / AdamW: the step count of this update (>= 1); SGD: 1 on the first step, else 0 */
+  /* Adam only (its rounding of param * weight_decay depends on where an element sits in its parameter tensor, see
+   * DESIGN.md 2.4): the index within its parameter of the run's first element, and 1 if torch's fused Adam steps that
+   * parameter on its scalar path (numel not a multiple of 4, or not 16-byte aligned), else 0.  A run then lies within one
+   * parameter.  Ignored by the other kinds. */
+  uint64_t run_index[B2_OPT_MAX_RUNS];
+  uint8_t run_scalar[B2_OPT_MAX_RUNS];
+  b2_optim_group_t group[B2_OPT_MAX_GROUPS];
+} b2_optim_t;
+
+int b2_reduce_scatter_step(b2_comm_t* comm, size_t block, const b2_segment_t* segments, int n_segments, int mode, float scale,
+                           const b2_optim_t* opt, void* stream);
 
 /*
  * All-to-all, a bit-exact copy of bytes (any dtype): out[r] <- the recv_bytes[r] bytes rank r sends this rank, in[j] is what

@@ -410,6 +410,19 @@ cudaError_t launch_reduce_scatter(const CommDev& d, const Src& src, int grid, vo
   }
 }
 
+// The optimizer-fused reduce-scatter at the communicator's world size (fp32-bucket modes only).
+template <int MODE, int W = 2>
+cudaError_t launch_reduce_scatter_step(const CommDev& d, const Src& src, const OptDev& o, int grid, unsigned long long n,
+                                       unsigned long long block, float scale, cudaStream_t s) {
+  if constexpr (W > B2_MAX_WORLD) {
+    return cudaErrorInvalidValue;
+  } else {
+    if (d.world != W) return launch_reduce_scatter_step<MODE, W + 1>(d, src, o, grid, n, block, scale, s);
+    k_reduce_scatter_step<MODE, W><<<grid, kThreads, 0, s>>>(d, src, o, n, block, scale);
+    return cudaGetLastError();
+  }
+}
+
 template <int MODE>
 cudaError_t launch_local(const Src& src, void* buf, unsigned long long n, float scale, cudaStream_t s) {
   // TMA-staged path for 16 B-aligned buckets.  The ring needs several tiles per CTA to pay for its prologue, so it is
@@ -1151,6 +1164,113 @@ int b2_reduce_scatter_gather(b2_comm_t* c, void* out, size_t block, const b2_seg
     c->launches++;
     off += n;
   }
+  return B2_OK;
+}
+
+// b2_optim_t -> the kernels' OptDev: the hyper-parameters rounded to fp32 as ATen's fused launches round them, the runs
+// checked to tile [0, block).  `fn` names the call in the error texts.
+static int optim_table(const char* fn, const b2_optim_t* opt, size_t block, OptDev& o) {
+  if (!opt) return fail(B2_EINVAL, "%s: null optimizer", fn);
+  if (opt->kind != B2_OPT_SGD && opt->kind != B2_OPT_ADAM && opt->kind != B2_OPT_ADAMW)
+    return fail(B2_EINVAL, "%s: unknown optimizer kind %d", fn, opt->kind);
+  if (opt->n_groups <= 0 || opt->n_groups > B2_OPT_MAX_GROUPS)
+    return fail(B2_EINVAL, "%s: need 1..%d parameter groups (got %d)", fn, B2_OPT_MAX_GROUPS, opt->n_groups);
+  if (opt->n_runs <= 0 || opt->n_runs > B2_OPT_MAX_RUNS)
+    return fail(B2_EINVAL, "%s: need 1..%d runs (got %d)", fn, B2_OPT_MAX_RUNS, opt->n_runs);
+  if (block >= (1ull << 32)) return fail(B2_EINVAL, "%s: block of %zu elements (the runs are 32-bit)", fn, block);
+  const bool adam = opt->kind != B2_OPT_SGD;
+  bool momentum = false;
+  o.kind = opt->kind;
+  o.nrun = opt->n_runs;
+  for (int gi = 0; gi < B2_OPT_MAX_GROUPS; ++gi) {
+    OptGroupDev& g = o.g[gi];
+    g = OptGroupDev{};
+    if (gi >= opt->n_groups) continue;
+    const b2_optim_group_t& h = opt->group[gi];
+    g.lr = static_cast<float>(h.lr);
+    g.wd = static_cast<float>(h.weight_decay);
+    g.flags = (h.maximize ? B2_OPT_F_MAXIMIZE : 0);
+    if (adam) {
+      g.a = static_cast<float>(h.beta1);
+      g.b = static_cast<float>(h.beta2);
+      g.eps = static_cast<float>(h.eps);
+      g.lr_wd = g.lr * g.wd;  // fp32 product, as ATen's AdamW forms it
+    } else {
+      g.a = static_cast<float>(h.momentum);
+      g.b = 1.0f - static_cast<float>(h.dampening);  // fp32, as the fused SGD kernel forms it
+      g.flags |= (h.nesterov ? B2_OPT_F_NESTEROV : 0) | (h.momentum != 0.0 ? B2_OPT_F_MOMENTUM : 0);
+      momentum = momentum || h.momentum != 0.0;
+    }
+  }
+  if (!opt->param || ((adam || momentum) && !opt->state0) || (adam && !opt->state1))
+    return fail(B2_EINVAL, "%s: null parameter or state pointer", fn);
+  o.param = opt->param;
+  o.s0 = opt->state0 ? opt->state0 : opt->param;  // never dereferenced without momentum
+  o.s1 = opt->state1 ? opt->state1 : opt->param;
+  o.off = 0;
+  if (opt->run_begin[0] != 0 || opt->run_begin[opt->n_runs] != block)
+    return fail(B2_EINVAL, "%s: runs cover [%llu, %llu), the block is [0, %zu)", fn, (unsigned long long)opt->run_begin[0],
+                (unsigned long long)opt->run_begin[opt->n_runs], block);
+  for (int k = 0; k < opt->n_runs; ++k) {
+    if (opt->run_begin[k + 1] <= opt->run_begin[k]) return fail(B2_EINVAL, "%s: run %d is empty or out of order", fn, k);
+    const int gi = opt->run_group[k];
+    if (gi != B2_OPT_NO_GROUP && gi >= opt->n_groups) return fail(B2_EINVAL, "%s: run %d names group %d of %d", fn, k, gi, opt->n_groups);
+    o.begin[k] = static_cast<uint32_t>(opt->run_begin[k]);
+    o.group[k] = static_cast<uint8_t>(gi | (gi != B2_OPT_NO_GROUP && opt->run_scalar[k] ? kOptScalar : 0));
+    o.pidx[k] = static_cast<uint16_t>(opt->run_index[k] & 0xffffu);
+    o.step[k] = opt->run_step[k];
+  }
+  for (int k = opt->n_runs; k <= B2_OPT_MAX_RUNS; ++k) o.begin[k] = static_cast<uint32_t>(block);
+  for (int k = opt->n_runs; k < B2_OPT_MAX_RUNS; ++k) {
+    o.group[k] = B2_OPT_NO_GROUP;
+    o.pidx[k] = 0;
+    o.step[k] = 0.f;
+  }
+  return B2_OK;
+}
+
+int b2_reduce_scatter_step(b2_comm_t* c, size_t block, const b2_segment_t* segments, int n_segments, int mode, float scale,
+                           const b2_optim_t* opt, void* stream) {
+  if (mode != B2_F32_WIRE_BF16 && mode != B2_F32 && mode != B2_F32_WIRE_F16)
+    return fail(B2_EINVAL, "b2_reduce_scatter_step: mode %d (fp32 buckets only: modes 0, 1, 3)", mode);
+  if (block == 0) return B2_OK;
+  OptDev o;  // checked first: it needs no communicator
+  if (const int rc = optim_table("b2_reduce_scatter_step", opt, block, o)) return rc;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  const int W = c->d.world;
+  Src src;
+  if (const int rc = segment_table("b2_reduce_scatter_step", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  auto step = [&](auto m) -> cudaError_t {
+    constexpr int MODE = decltype(m)::value;
+    if (W == 1) {  // the local pass's grid and rounding
+      const unsigned long long V = (block + 7) / 8;
+      unsigned long long grid = (V + kThreads * 4ull - 1) / (kThreads * 4ull);
+      const unsigned long long cap = 4ull * static_cast<unsigned long long>(sm_count(c->device));
+      grid = grid < 1 ? 1 : (grid > cap ? cap : grid);
+      k_local_step<MODE><<<static_cast<int>(grid), kThreads, 0, s>>>(src, o, block, scale);
+      c->launches++;
+      return cudaGetLastError();
+    }
+    const size_t cap = c->d.slice_cap / dev::Wire<MODE>::kBytes * 8;  // elements of a block one recv region holds
+    for (size_t off = 0; off < block;) {
+      const size_t n = block - off < cap ? block - off : cap;
+      src.off = off;  // the same block offset for the gradient table and the parameter / state slices
+      o.off = off;
+      const cudaError_t e = launch_reduce_scatter_step<MODE>(c->d, src, o, grid_for(c, (n + 7) / 8, 1), n, block, scale, s);
+      if (e != cudaSuccess) return e;
+      c->launches++;
+      off += n;
+    }
+    return cudaSuccess;
+  };
+  cudaError_t e = cudaErrorInvalidValue;
+  if (mode == B2_F32_WIRE_BF16) e = step(std::integral_constant<int, B2_F32_WIRE_BF16>{});
+  else if (mode == B2_F32) e = step(std::integral_constant<int, B2_F32>{});
+  else e = step(std::integral_constant<int, B2_F32_WIRE_F16>{});
+  if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter step kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 

@@ -3,6 +3,7 @@
 #pragma once
 
 #include "b2_dev.cuh"
+#include "b2_optim.cuh"
 
 // W == 1 (and the single-GPU roofline probe): x <- round(wire(scale * x)), one streaming pass.  Each CTA owns a contiguous
 // range of vecs and a thread's successive vecs are 512 apart (a warp still reads 1 KiB of consecutive memory per access):
@@ -35,6 +36,31 @@ __global__ void __launch_bounds__(kThreads) k_local_pass(const __grid_constant__
         store_out<MODE>(buf, v * 8, n, aligned, finalize<MODE>(widen<MODE>(c)));
       }
     }
+  }
+}
+
+// W == 1 with the optimizer step (b2_reduce_scatter_step): the local pass's rounding of each vec read through the segment
+// table (mode 0 is not a copy: it rounds to bf16), then the optimizer epilogue on the parameter and state slices
+// (b2_optim.cuh) instead of the store.  The local pass's CTA layout, so a thread's segment and run hints keep hitting.
+template <int MODE>
+__global__ void __launch_bounds__(kThreads, 1) k_local_step(const __grid_constant__ Src src, const __grid_constant__ OptDev o,
+                                                         unsigned long long n, float scale) {
+  using namespace dev;
+  __shared__ OptCta t;
+  opt_cta_init(o, t);
+  __syncthreads();
+  const unsigned long long V = (n + 7) / 8;
+  constexpr unsigned long long kTrip = static_cast<unsigned long long>(kThreads) * 4;
+  const unsigned long long per_cta = (V + gridDim.x - 1) / gridDim.x;
+  const unsigned long long span = (per_cta + kTrip - 1) / kTrip * kTrip;
+  const unsigned long long lo = blockIdx.x * span;
+  const unsigned long long hi = lo + span < V ? lo + span : V;
+  SegHint hint;
+  RunHint rh;
+  for (unsigned long long v = lo + threadIdx.x; v < hi; v += kThreads) {
+    const F8 x = load_src<MODE>(src, hint, nullptr, v * 8, n, false);
+    const Wire<MODE> c = compress<MODE>(x, scale);
+    opt_step_vec(o, t, rh, v * 8, n, widen<MODE>(finalize<MODE>(widen<MODE>(c))));
   }
 }
 

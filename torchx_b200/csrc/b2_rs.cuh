@@ -18,24 +18,20 @@
 
 #include "b2_dev.cuh"
 #include "b2_exact.cuh"
+#include "b2_optim.cuh"
 
-// Float SUM / AVG: out <- round(sum_r wire(scale * in_r[rank block])), the rank-order fp32 sum of k_twoshot.
+// Phase A of the float kernels: block j of my input -> recv[me] of rank j, as wire(scale * x).
 template <int MODE, int W>
-__global__ void __launch_bounds__(kThreads, 1)
-    k_reduce_scatter(CommDev c, const __grid_constant__ Src src, void* out, const void* in, unsigned long long n,
-                     unsigned long long block, float scale) {
+__device__ __forceinline__ void rs_scatter(const CommDev& c, const Src& src, const void* in, unsigned long long n,
+                                           unsigned long long block, float scale, unsigned long long stage) {
   using namespace dev;
   using Elem = typename ModeTraits<MODE>::Elem;
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
-  const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
   const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
   const unsigned long long my_recv = stage + c.rank * c.slice_cap;
-
-  // ---- phase A -------------------------------------------------------------------------------
   for (unsigned long long v0 = first; v0 < V; v0 += stride * U) {
     F8 x[U][W];
 #pragma unroll
@@ -56,6 +52,24 @@ __global__ void __launch_bounds__(kThreads, 1)
         if (v < V) st_wire<MODE>(c.peer[jj] + my_recv + v * WVB, compress<MODE>(x[u][jj], scale));
     }
   }
+}
+
+// Float SUM / AVG: out <- round(sum_r wire(scale * in_r[rank block])), the rank-order fp32 sum of k_twoshot.
+template <int MODE, int W>
+__global__ void __launch_bounds__(kThreads, 1)
+    k_reduce_scatter(CommDev c, const __grid_constant__ Src src, void* out, const void* in, unsigned long long n,
+                     unsigned long long block, float scale) {
+  using namespace dev;
+  constexpr int WVB = Wire<MODE>::kBytes;
+  constexpr int U = vecs_per_trip(W);
+  const uint32_t seq0 = op_begin(c);
+  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long V = (n + 7) / 8;
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
+  const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
+
+  // ---- phase A -------------------------------------------------------------------------------
+  rs_scatter<MODE, W>(c, src, in, n, block, scale, stage);
   cta_xbar(c, seq0 * 4u + 1u);
 
   // ---- phase B -------------------------------------------------------------------------------
@@ -79,6 +93,38 @@ __global__ void __launch_bounds__(kThreads, 1)
         store_out<MODE>(out, v * 8, n, aligned, finalize<MODE>(s));
       }
     }
+  }
+  op_end(c, seq0);
+}
+
+// The same reduce-scatter with the optimizer step as its phase B epilogue (b2_reduce_scatter_step, b2_optim.cuh): the
+// reduced vec is rounded as `out` would hold it, then steps this rank's parameter and state slices at the same block
+// offset.  Phase B runs one vec per trip: the epilogue's three loads and stores per element need the registers.
+template <int MODE, int W>
+__global__ void __launch_bounds__(kThreads, 1)
+    k_reduce_scatter_step(CommDev c, const __grid_constant__ Src src, const __grid_constant__ OptDev o, unsigned long long n,
+                          unsigned long long block, float scale) {
+  using namespace dev;
+  constexpr int WVB = Wire<MODE>::kBytes;
+  __shared__ OptCta t;
+  const uint32_t seq0 = op_begin(c);
+  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long V = (n + 7) / 8;
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
+  const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
+  opt_cta_init(o, t);  // visible to every thread after cta_xbar's barriers
+
+  rs_scatter<MODE, W>(c, src, nullptr, n, block, scale, stage);
+  cta_xbar(c, seq0 * 4u + 1u);
+
+  const uint8_t* mine = c.peer[0] + stage;
+  RunHint h;
+  for (unsigned long long v = first; v < V; v += stride) {
+    Wire<MODE> w[W];
+#pragma unroll
+    for (int r = 0; r < W; ++r) w[r] = ld_wire<MODE>(mine + r * c.slice_cap + v * WVB);
+    const F8 s = reduce_rank_order<MODE, W>(w);
+    opt_step_vec(o, t, h, v * 8, n, widen<MODE>(finalize<MODE>(s)));
   }
   op_end(c, seq0);
 }

@@ -93,6 +93,7 @@ SYMBOLS = [
     "b2_allgather",
     "b2_reduce_scatter",
     "b2_reduce_scatter_gather",
+    "b2_reduce_scatter_step",
     "b2_alltoall",
     "b2_alltoall_max_bytes",
     "b2_batchnorm_stats",
@@ -110,6 +111,32 @@ class B2Segment(ctypes.Structure):
     """b2_segment_t: bucket elements [begin, end) live at device pointer src."""
 
     _fields_ = [("src", ctypes.c_void_p), ("begin", ctypes.c_uint64), ("end", ctypes.c_uint64)]
+
+
+B2_OPT_SGD = 1
+B2_OPT_ADAM = 2
+B2_OPT_ADAMW = 3
+B2_OPT_MAX_GROUPS = 8
+B2_OPT_MAX_RUNS = 128
+B2_OPT_NO_GROUP = 255
+
+
+class B2OptimGroup(ctypes.Structure):
+    """b2_optim_group_t: one parameter group's hyper-parameters, as the optimizer's param_groups hold them."""
+
+    _fields_ = [("lr", ctypes.c_double), ("weight_decay", ctypes.c_double), ("momentum", ctypes.c_double),
+                ("dampening", ctypes.c_double), ("beta1", ctypes.c_double), ("beta2", ctypes.c_double),
+                ("eps", ctypes.c_double), ("nesterov", ctypes.c_int), ("maximize", ctypes.c_int)]
+
+
+class B2Optim(ctypes.Structure):
+    """b2_optim_t: the optimizer step fused into b2_reduce_scatter_step."""
+
+    _fields_ = [("kind", ctypes.c_int), ("n_groups", ctypes.c_int), ("n_runs", ctypes.c_int),
+                ("param", ctypes.c_void_p), ("state0", ctypes.c_void_p), ("state1", ctypes.c_void_p),
+                ("run_begin", ctypes.c_uint64 * (B2_OPT_MAX_RUNS + 1)), ("run_group", ctypes.c_uint8 * B2_OPT_MAX_RUNS),
+                ("run_step", ctypes.c_float * B2_OPT_MAX_RUNS), ("run_index", ctypes.c_uint64 * B2_OPT_MAX_RUNS),
+                ("run_scalar", ctypes.c_uint8 * B2_OPT_MAX_RUNS), ("group", B2OptimGroup * B2_OPT_MAX_GROUPS)]
 
 
 class B2Error(RuntimeError):
@@ -189,6 +216,8 @@ def lib() -> ctypes.CDLL:
     L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
     L.b2_reduce_scatter_gather.restype = i
     L.b2_reduce_scatter_gather.argtypes = [vp, vp, sz, ctypes.POINTER(B2Segment), i, i, f, vp]
+    L.b2_reduce_scatter_step.restype = i
+    L.b2_reduce_scatter_step.argtypes = [vp, sz, ctypes.POINTER(B2Segment), i, i, f, ctypes.POINTER(B2Optim), vp]
     L.b2_alltoall.restype = i
     L.b2_alltoall.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(vp), ctypes.POINTER(sz), vp]
     L.b2_alltoall_max_bytes.restype = sz

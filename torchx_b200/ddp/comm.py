@@ -261,6 +261,20 @@ class Communicator:
                                                  ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return out
 
+    def reduce_scatter_step_(self, block: int, segments, n_segments: int, opt, scale: Optional[float] = None,
+                             wire: str = "bf16", stream: Optional[torch.cuda.Stream] = None) -> None:
+        """``reduce_scatter_gather_`` with the optimizer step fused in (include/b200ddp.h: b2_reduce_scatter_step): the
+        reduced block steps this rank's block of the flat fp32 parameter buffer and its optimizer state as ``opt`` (a
+        ``_native.B2Optim``) describes them, with the arithmetic of torch's fused SGD / Adam / AdamW.  The overlap mode of
+        the sharded mini-DDP."""
+        if scale is None:
+            scale = 1.0 / self.world
+        mode = _MODE_FOR.get(("f32", wire))
+        if mode is None:
+            raise ValueError(f"unsupported wire format {wire!r}")
+        N.check(N.lib().b2_reduce_scatter_step(self._h, block, segments, n_segments, mode, ctypes.c_float(scale),
+                                               ctypes.byref(opt), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+
     def alltoall_(self, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor],
                   stream: Optional[torch.cuda.Stream] = None) -> Sequence[torch.Tensor]:
         """``outs[r]`` <- the ``ins[rank]`` of rank r, bit for bit (include/b200ddp.h: b2_alltoall).  Both are lists of world

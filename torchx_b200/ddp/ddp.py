@@ -71,7 +71,7 @@ class _Bucket:
                 self.segments[i].end = o + n
         self.block = 0  # sharded mode (ZeroRedundancyOptimizer): elements of this rank's shard, else 0
 
-    def shard(self, world: int, device: torch.device) -> None:
+    def shard(self, world: int, device: torch.device, grad_shard: bool = True) -> None:
         """Switch to the ZeRO-1 layout: the bucket is padded to world * block elements, the parameters move into one
         persistent flat buffer of that size, and the full-size gradient bucket gives way to this rank's block-sized
         gradient shard.  The pad reads as zero through a last segment that points at a small zero tensor."""
@@ -87,7 +87,8 @@ class _Bucket:
                 v = _view_like(self.param_flat[o : o + n], p)  # the parameter's own strides: channels_last stays so
                 v.copy_(p.data)
                 p.data = v
-        self.shard_grad = torch.zeros(self.block, dtype=self.dtype, device=device)
+        # no gradient shard when the optimizer step runs inside the reduce-scatter (overlap_with_ddp)
+        self.shard_grad = torch.zeros(self.block, dtype=self.dtype, device=device) if grad_shard else None
         self.pad_zeros = torch.zeros(max(pad, 1), dtype=self.dtype, device=device)
 
         def table(ranges):
@@ -161,6 +162,7 @@ class DistributedDataParallel(nn.Module):
         self.sharded = False         # ZeRO-1 layout (ZeroRedundancyOptimizer): each rank keeps one block of every bucket
         self._shard_grads: List = []  # (optimizer view, its gradient shard view): attached after every synced backward
         self._shard_grads_live = False  # the shards hold a reduced gradient that zero_grad() has not cleared
+        self._step_in_backward = None  # a ZeroRedundancyOptimizer(overlap_with_ddp=True): each bucket launch steps it
         self._synced_backwards = 0
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad_ready) for p in self._params]
         # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen
@@ -204,15 +206,20 @@ class DistributedDataParallel(nn.Module):
             if bufs:
                 self._broadcast_coalesced(bufs)
 
-    def _enable_sharding(self) -> None:
-        """The ZeRO-1 layout of every bucket (_Bucket.shard); ZeroRedundancyOptimizer's constructor calls it."""
+    def _check_shardable(self) -> None:
         if self.sharded:
             raise RuntimeError("this DistributedDataParallel is already sharded by a ZeroRedundancyOptimizer")
         if self._synced_backwards:
             raise RuntimeError("ZeroRedundancyOptimizer must be constructed before the model's first backward")
+
+    def _enable_sharding(self, step_in_backward=None) -> None:
+        """The ZeRO-1 layout of every bucket (_Bucket.shard); ZeroRedundancyOptimizer's constructor calls it.  With
+        ``step_in_backward`` (an overlap_with_ddp optimizer) every bucket launch also steps that optimizer's shard."""
+        self._check_shardable()
         for b in self.buckets:
-            b.shard(self.world_size, self.device)
+            b.shard(self.world_size, self.device, grad_shard=step_in_backward is None)
         self.sharded = True
+        self._step_in_backward = step_in_backward
 
     # ---- training step -----------------------------------------------------------------------------
     def _reset_reducer_state(self) -> None:
@@ -312,6 +319,13 @@ class DistributedDataParallel(nn.Module):
         """Sharded mode: reduce-scatter the bucket (padded to W blocks) into this rank's gradient shard, with the wire,
         scale, order and stream of the allreduce.  Its gradients are read in place, or copied into one scratch tensor
         first when they cannot be (more segments than a table holds, another layout, zero_copy=False)."""
+        zero = self._step_in_backward
+        if self._next_bucket == 0 and zero is not None and zero._stepped_in_backward:
+            # the parameters of this rank's blocks already hold the update of the previous backward: a second update
+            # before step() all-gathers it would step from a half-updated model.  Raised before any bucket is launched.
+            raise RuntimeError(
+                "a second synced backward before step(): with overlap_with_ddp=True each synced backward updates the "
+                "parameters; call step() after every synced backward, and accumulate micro-batches under no_sync()")
         if self._next_bucket == 0 and self._shard_grads_live:
             # Unsharded, this backward would add into the reduced gradients still in p.grad.  The sharded gradients live
             # only in the shards, which this backward overwrites: refuse rather than drop the earlier micro-batch.  (Raised
@@ -338,8 +352,12 @@ class DistributedDataParallel(nn.Module):
             t0 = torch.cuda.Event(enable_timing=True)
             t0.record(self._comm_stream)
         # the gradients (and the scratch copy) stay referenced until _finalize_backward has made the compute stream wait
-        self.comm.reduce_scatter_gather_(b.shard_grad, segs, len(segs), scale=1.0 / self.world_size, wire=self.wire,
-                                         stream=self._comm_stream)
+        if zero is not None:  # hyper-parameters read now: a scheduler stepped after step() reaches the next backward
+            self.comm.reduce_scatter_step_(b.block, segs, len(segs), zero._launch_table(b), scale=1.0 / self.world_size,
+                                           wire=self.wire, stream=self._comm_stream)
+        else:
+            self.comm.reduce_scatter_gather_(b.shard_grad, segs, len(segs), scale=1.0 / self.world_size, wire=self.wire,
+                                             stream=self._comm_stream)
         b.done.record(self._comm_stream)
         if self._profile is not None:
             t1 = torch.cuda.Event(enable_timing=True)
@@ -368,6 +386,8 @@ class DistributedDataParallel(nn.Module):
             for v, g in self._shard_grads:
                 v.grad = g
             self._shard_grads_live = bool(self._shard_grads)
+            if self._step_in_backward is not None:
+                self._step_in_backward._stepped_in_backward = True
             self._synced_backwards += 1
             self.comm.check()
         finally:

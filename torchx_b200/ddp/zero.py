@@ -17,6 +17,7 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
+from . import _native as N
 from .ddp import DistributedDataParallel, _view_like
 
 # the elementwise optimizers: a slice of a tensor steps to the bits of the same slice of the stepped tensor
@@ -41,6 +42,49 @@ def block_intersections(offsets: Sequence[int], numels: Sequence[int], block: in
     return out
 
 
+def block_runs(offsets: Sequence[int], numels: Sequence[int], groups: Sequence[int], block: int,
+               rank: int) -> List[Tuple[int, int, int, Optional[int]]]:
+    """(lo, hi, group, index) tiling rank's block [0, block) in block coordinates: the part of parameter ``index`` (of
+    parameter group ``group``) there, then the pad as (lo, block, B2_OPT_NO_GROUP, None), which is never stepped."""
+    runs: List[Tuple[int, int, int, Optional[int]]] = [
+        (lo - rank * block, hi - rank * block, groups[i], i) for i, lo, hi in block_intersections(offsets, numels, block, rank)]
+    end = runs[-1][1] if runs else 0
+    if end < block:
+        runs.append((end, block, N.B2_OPT_NO_GROUP, None))
+    return runs
+
+
+def launch_runs(runs: Sequence[tuple], sgd: bool) -> List[Tuple[int, int, float, Optional[Tuple[int, bool]]]]:
+    """(begin, group, step, pos) of one launch from (begin, group, steps taken or None for the pad[, pos]): the step a run's
+    update uses (Adam: steps taken + 1; SGD: 1.0 on the first step, else 0.0; the pad: 0.0), adjacent equal runs
+    coalesced.  ``pos`` = (index within its parameter of the run's first element, the parameter takes the fused Adam's
+    scalar path) marks a run whose rounding depends on where its elements sit in their parameter (Adam's coupled weight
+    decay, DESIGN.md 2.4): such a run is never merged."""
+    out: List[Tuple[int, int, float, Optional[Tuple[int, bool]]]] = []
+    for lo, gi, n, *rest in runs:
+        pos = rest[0] if rest else None
+        step = 0.0 if n is None else (float(n == 0) if sgd else float(n + 1))
+        if pos is None and out and out[-1][1] == gi and out[-1][2] == step and out[-1][3] is None:
+            continue
+        out.append((lo, gi, step, pos))
+    return out
+
+
+def _check_run_bound(groups: Sequence[Sequence[int]], counts: Sequence[Sequence[int]], sgd: bool,
+                     distinct: Optional[Sequence[Sequence[bool]]] = None) -> None:
+    """Overlap mode: every launch's run table fits B2_OPT_MAX_RUNS.  A rank's block holds at most the runs of the whole
+    bucket (adjacent parameters of one group and step coalesced) plus the pad, whatever W and the rank: checked from the
+    bucket layout alone, so every rank reaches the same decision before any bucket is launched."""
+    for bi, (gs, cs) in enumerate(zip(groups, counts)):
+        ds = distinct[bi] if distinct is not None else [False] * len(gs)
+        n = len(launch_runs([(0, g, c, (0, False) if d else None) for g, c, d in zip(gs, cs, ds)], sgd)) + 1
+        if n > N.B2_OPT_MAX_RUNS:
+            raise ValueError(
+                f"overlap_with_ddp=True: bucket {bi} alternates between parameter groups (or step counts) {n - 1} times; the "
+                f"fused step's run table holds {N.B2_OPT_MAX_RUNS - 1} runs and the pad.  Use a smaller bucket_cap_mb or "
+                "order the parameters so that each group's are adjacent")
+
+
 def _ordered(comm: Any, launch) -> None:
     from torchx_b200.nn.batchnorm import _ordered as ordered
 
@@ -61,7 +105,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
 
     _step_supports_amp_scaling = True  # GradScaler hands itself to step(): the found-inf decision is made rank-global there
 
-    def __init__(self, model: DistributedDataParallel, optimizer_class: type, params: Optional[Any] = None, **defaults: Any) -> None:
+    def __init__(self, model: DistributedDataParallel, optimizer_class: type, params: Optional[Any] = None,
+                 overlap_with_ddp: bool = False, **defaults: Any) -> None:
         if optimizer_class not in SUPPORTED:
             raise TypeError(f"ZeroRedundancyOptimizer supports {', '.join(c.__name__ for c in SUPPORTED)}, "
                             f"not {getattr(optimizer_class, '__name__', optimizer_class)}")
@@ -69,12 +114,21 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             raise TypeError("ZeroRedundancyOptimizer shards a torchx_b200.ddp.DistributedDataParallel")
         groups = _normalize_groups(model._params if params is None else params)
         _check_groups(groups, model._params)
+        if overlap_with_ddp:
+            model._check_shardable()
+            _check_overlap(groups, defaults, model)
+            gi_of = {id(p): gi for gi, g in enumerate(groups) for p in g["params"]}
+            pos = [optimizer_class is torch.optim.Adam and bool({**defaults, **g}.get("weight_decay", 0)) for g in groups]
+            _check_run_bound([[gi_of[id(p)] for p in b.params] for b in model.buckets],
+                             [[0] * len(b.params) for b in model.buckets], optimizer_class is torch.optim.SGD,
+                             [[pos[gi_of[id(p)]] for p in b.params] for b in model.buckets])
         super().__init__(groups, defaults)  # validates the groups and fills in the defaults
         self.model = model
         self.comm = model.comm
         self.optimizer_class = optimizer_class
+        self.overlap_with_ddp = overlap_with_ddp
         self._full_groups = [list(g["params"]) for g in self.param_groups]  # model parameters, the user's order
-        model._enable_sharding()
+        model._enable_sharding(self if overlap_with_ddp else None)
 
         W, r = model.world_size, self.comm.rank
         where: Dict[int, Tuple[Any, int, int]] = {}  # id(param) -> (bucket, offset, numel)
@@ -88,7 +142,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             for i, lo, hi in block_intersections(b.spec.offsets, b.spec.numels, b.block, r):
                 v = b.param_flat[lo:hi]
                 self._views[id(b.params[i])] = (v, lo, hi)
-                model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block]))
+                if not overlap_with_ddp:
+                    model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block]))
         inner_groups = []
         for g, ps in zip(self.param_groups, self._full_groups):
             inner = {k: val for k, val in g.items() if k != "params"}
@@ -100,6 +155,87 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         self.defaults = self.optim.defaults
         self._world, self._rank = W, r
         self._stepped = False  # the same on every rank: the skip decision under a GradScaler is rank-global
+        self._stepped_in_backward = False  # overlap mode: a synced backward has updated this rank's blocks since step()
+        if overlap_with_ddp:
+            self._init_overlap()
+
+    # ---- overlap_with_ddp: the step inside each bucket's reduce-scatter ---------------------------------------------
+    def _init_overlap(self) -> None:
+        """Flat per-bucket state buffers of ``block`` elements, which the kernel indexes like this rank's parameter block;
+        the inner optimizer's per-parameter state entries are views into them, so checkpoints see the usual layout."""
+        sgd = self.optimizer_class is torch.optim.SGD
+        self._state_keys = ["momentum_buffer"] if sgd else ["exp_avg", "exp_avg_sq"]
+        self._kind = N.B2_OPT_SGD if sgd else (N.B2_OPT_ADAM if self.optimizer_class is torch.optim.Adam else N.B2_OPT_ADAMW)
+        group_of = {id(p): gi for gi, ps in enumerate(self._full_groups) for p in ps}
+        dev, r = self.model.device, self._rank
+        self._flat_state: Dict[int, Dict[str, torch.Tensor]] = {}
+        self._runs: Dict[int, List[Tuple[int, int, int, Optional[torch.Tensor]]]] = {}
+        self._count: Dict[int, int] = {}  # id(view) -> steps taken (host copy of the `step` state, no device sync)
+        self._pos: Dict[int, Tuple[int, bool]] = {}  # id(view) -> (index in its parameter of its first element, scalar path)
+        for bi, b in enumerate(self.model.buckets):
+            flat = {k: torch.zeros(b.block, dtype=torch.float32, device=dev) for k in self._state_keys}
+            self._flat_state[bi] = flat
+            runs = []
+            for lo, hi, gi, i in block_runs(b.spec.offsets, b.spec.numels, [group_of[id(p)] for p in b.params], b.block, r):
+                v = self._views[id(b.params[i])][0] if i is not None else None
+                runs.append((lo, hi, gi, v))
+                if v is not None:  # where the run starts in its parameter, and whether the fused Adam's path is the scalar one
+                    self._pos[id(v)] = (lo + r * b.block - b.spec.offsets[i], b.spec.numels[i] % 4 != 0)
+                if v is not None:
+                    self._count[id(v)] = 0
+            self._runs[bi] = runs
+        self._bucket_index = {id(b): bi for bi, b in enumerate(self.model.buckets)}
+        self._attach_state()
+
+    def _attach_state(self) -> None:
+        """state[view] <- views of the flat buffers (and a device fp32 ``step``, as the fused optimizers keep it)."""
+        for bi, runs in self._runs.items():
+            for lo, hi, gi, v in runs:
+                if v is None:
+                    continue
+                g = self.param_groups[gi]
+                st: Dict[str, Any] = {}
+                if self.optimizer_class is torch.optim.SGD:
+                    if g["momentum"] != 0:
+                        st["momentum_buffer"] = self._flat_state[bi]["momentum_buffer"][lo:hi]
+                else:
+                    st["step"] = torch.tensor(float(self._count[id(v)]), dtype=torch.float32, device=self.model.device)
+                    st["exp_avg"] = self._flat_state[bi]["exp_avg"][lo:hi]
+                    st["exp_avg_sq"] = self._flat_state[bi]["exp_avg_sq"][lo:hi]
+                self.optim.state[v] = st
+
+    def _launch_table(self, b) -> "N.B2Optim":
+        """The b2_optim_t of one bucket launch: this rank's parameter and state blocks, its runs (adjacent parameters of
+        one group and step count coalesced) and every group's hyper-parameters as param_groups hold them now."""
+        bi = self._bucket_index[id(b)]
+        t = N.B2Optim()
+        t.kind = self._kind
+        t.n_groups = len(self.param_groups)
+        t.param = b.param_flat[self._rank * b.block :].data_ptr()
+        flat = self._flat_state[bi]
+        t.state0 = flat[self._state_keys[0]].data_ptr()
+        t.state1 = flat["exp_avg_sq"].data_ptr() if "exp_avg_sq" in flat else None
+        sgd = self._kind == N.B2_OPT_SGD
+        for gi, g in enumerate(self.param_groups):
+            h = t.group[gi]
+            h.lr, h.weight_decay, h.maximize = float(g["lr"]), float(g["weight_decay"]), int(bool(g["maximize"]))
+            if sgd:
+                h.momentum, h.dampening, h.nesterov = float(g["momentum"]), float(g["dampening"]), int(bool(g["nesterov"]))
+            else:
+                h.beta1, h.beta2 = float(g["betas"][0]), float(g["betas"][1])
+                h.eps = float(g["eps"])
+        pos_groups = {gi for gi, g in enumerate(self.param_groups) if self._kind == N.B2_OPT_ADAM and g["weight_decay"]}
+        runs = launch_runs([(lo, gi, self._count[id(v)] if v is not None else None,
+                             self._pos[id(v)] if v is not None and gi in pos_groups else None)
+                            for lo, _, gi, v in self._runs[bi]], sgd)
+        assert len(runs) <= N.B2_OPT_MAX_RUNS, "bounded by _check_run_bound at construction and on load"
+        t.n_runs = len(runs)
+        for k, (lo, gi, step, pos) in enumerate(runs):
+            t.run_begin[k], t.run_group[k], t.run_step[k] = lo, gi, step
+            if pos is not None:
+                t.run_index[k], t.run_scalar[k] = pos
+        t.run_begin[len(runs)] = b.block
+        return t
 
     # ---- step ------------------------------------------------------------------------------------
     @torch.no_grad()
@@ -114,6 +250,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         apart.  Should torch drop the keyword, ``step()`` stops being called with it and a GradScaler run raises below."""
         if closure is not None:
             raise RuntimeError("ZeroRedundancyOptimizer.step does not take a closure")
+        if self.overlap_with_ddp:
+            return self._step_overlap(grad_scaler)
         if grad_scaler is None and getattr(self, "found_inf", None) is not None:
             raise RuntimeError("this GradScaler no longer passes itself to step(): the rank-global inf check cannot run")
         if grad_scaler is not None:
@@ -130,6 +268,30 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             if sum(t.item() for t in found.values()):
                 return None
         self.optim.step()
+        self._stepped = True
+        for b in self.model.buckets:
+            own = b.param_flat[self._rank * b.block : (self._rank + 1) * b.block]
+            _ordered(self.comm, lambda s, b=b, own=own: self.comm.allgather_(b.param_flat, own, stream=s))
+        return None
+
+    def _step_overlap(self, grad_scaler) -> None:
+        """The update already ran inside the backward's reduce-scatters: all-gather every bucket's parameter buffer and
+        advance the step counts.  A no-op without a synced backward since the previous step()."""
+        if grad_scaler is not None or getattr(self, "found_inf", None) is not None:
+            raise RuntimeError(
+                "overlap_with_ddp=True does not support GradScaler: dynamic loss scaling needs the rank-global found-inf "
+                "before any update, and with overlap the update has already happened during backward")
+        if not self._stepped_in_backward:
+            return None
+        self._stepped_in_backward = False
+        steps = []
+        for k in self._count:
+            self._count[k] += 1
+        for st in self.optim.state.values():
+            if "step" in st:
+                steps.append(st["step"])
+        if steps:
+            torch._foreach_add_(steps, 1.0)
         self._stepped = True
         for b in self.model.buckets:
             own = b.param_flat[self._rank * b.block : (self._rank + 1) * b.block]
@@ -157,6 +319,9 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         """Clips the sharded gradients in place by their global 2-norm and returns that norm (fp32, the same bits on
         every rank): the sqrt of the rank-order fp32 sum of each rank's fp32 sum of squares over its shard.  The clip
         coefficient is torch's, ``max_norm / (norm + 1e-6)`` clamped to 1."""
+        if self.overlap_with_ddp:
+            raise RuntimeError("overlap_with_ddp=True does not support clip_grad_norm_: the update has already happened "
+                               "during backward, before a global norm could be known")
         dev = self.model.device
         grads = [v.grad for v, _ in self.model._shard_grads if v.grad is not None]
         sq = torch.zeros(1, dtype=torch.float32, device=dev)
@@ -252,6 +417,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         groups = state_dict["param_groups"]
         if len(groups) != len(self._full_groups) or any(len(g["params"]) != len(ps) for g, ps in zip(groups, self._full_groups)):
             raise ValueError("the state dict's param groups do not match this optimizer's")
+        if self.overlap_with_ddp:
+            self._check_loaded_runs(state_dict)
         inner_state: Dict[int, Dict[str, Any]] = {}
         inner_groups, at = [], 0
         for g, ps in zip(groups, self._full_groups):
@@ -278,6 +445,67 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         self._stepped = bool(state_dict["state"])
         self.param_groups = self.optim.param_groups
         self.state = self.optim.state
+        if self.overlap_with_ddp:
+            self._land_loaded_state()
+
+    def _check_loaded_runs(self, state_dict: Dict[str, Any]) -> None:
+        """Overlap mode, before loading: the run bound with the checkpoint's step counts (the same on every rank)."""
+        index = {id(p): i for i, p in enumerate(self._index())}
+        gi_of = {id(p): gi for gi, ps in enumerate(self._full_groups) for p in ps}
+        sgd = self.optimizer_class is torch.optim.SGD
+
+        def count(p):
+            st = state_dict["state"].get(index[id(p)], {})
+            return int(float(st["step"])) if "step" in st else int(bool(st))
+
+        pos = [self._kind == N.B2_OPT_ADAM and bool(g["weight_decay"]) for g in self.param_groups]
+        _check_run_bound([[gi_of[id(p)] for p in b.params] for b in self.model.buckets],
+                         [[count(p) for p in b.params] for b in self.model.buckets], sgd,
+                         [[pos[gi_of[id(p)]] for p in b.params] for b in self.model.buckets])
+
+    @torch.no_grad()
+    def _land_loaded_state(self) -> None:
+        """Overlap mode: the loaded per-parameter state goes into the flat buffers the kernel steps, and the state entries
+        become views of them again; the host step counts follow the loaded ``step`` (read once, here)."""
+        loaded = {id(v): st for v, st in self.optim.state.items()}
+        for flat in self._flat_state.values():
+            for t in flat.values():
+                t.zero_()
+        for bi, runs in self._runs.items():
+            for lo, hi, gi, v in runs:
+                if v is None:
+                    continue
+                st = loaded.get(id(v), {})
+                for k in self._state_keys:
+                    if k in st:
+                        self._flat_state[bi][k][lo:hi].copy_(st[k].reshape(-1))
+                if "step" in st:
+                    self._count[id(v)] = int(float(st["step"]))
+                else:
+                    self._count[id(v)] = 1 if st else 0
+        self.optim.state.clear()
+        self._attach_state()
+
+
+def _check_overlap(groups: List[Dict[str, Any]], defaults: Dict[str, Any], model: DistributedDataParallel) -> None:
+    """What the fused step inside the reduce-scatter cannot do, refused before anything is sharded."""
+    if model.wire not in ("bf16", "f32", "f16"):
+        raise ValueError(f"overlap_with_ddp=True: unknown wire format {model.wire!r}")
+    if any(p.dtype != torch.float32 for p in model._params):
+        raise TypeError("overlap_with_ddp=True steps fp32 parameters only (modes B2_F32_WIRE_BF16, B2_F32, B2_F32_WIRE_F16)")
+    if len(groups) > N.B2_OPT_MAX_GROUPS:
+        raise ValueError(f"overlap_with_ddp=True takes at most {N.B2_OPT_MAX_GROUPS} parameter groups, got {len(groups)}")
+    for g in groups:
+        opts = {**defaults, **{k: v for k, v in g.items() if k != "params"}}
+        if opts.get("amsgrad"):
+            raise ValueError("overlap_with_ddp=True does not support amsgrad")
+        if torch.is_tensor(opts.get("lr")):
+            raise TypeError("overlap_with_ddp=True needs a float lr, not a tensor")
+        if opts.get("foreach"):
+            raise ValueError("overlap_with_ddp=True runs its own fused step: foreach=True does not apply")
+        for k in ("capturable", "differentiable"):
+            if opts.get(k):
+                raise ValueError(f"overlap_with_ddp=True does not support {k}=True")
 
 
 def _owns(where, rank: int) -> bool:
