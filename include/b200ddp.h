@@ -47,7 +47,8 @@ extern "C" {
 #endif
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
-                            b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall* and b2_reduce_scatter_step, which only add symbols: a binding that needs them
+                            b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats
+                            and b2_bn_backward_reduce, which only add symbols: a binding that needs them
                             fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -384,6 +385,28 @@ int b2_bn_forward_elemt(const void* x, void* y, size_t rows, size_t channels, in
 int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
                          const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, int device,
                          void* stream);
+
+/*
+ * The two reductions of training-mode BatchNorm2d on the same [rows, channels] view, with the bits of ATen's channels-last
+ * kernels (batch_norm_collect_statistics_channels_last_kernel and the running-statistics update of batch_norm_update_stats;
+ * batch_norm_backward_reduce_channels_last_kernel): the same reduction tree, order and contractions (DESIGN.md 2.4).  They
+ * cover the inputs ATen reduces with those kernels: rows * channels < 2^31 - 1 (B2_EINVAL above), plus the checks of the
+ * elementwise passes.  A layer whose tree has more than one CTA row (geometry[3] > 1) needs a float-aligned device
+ * workspace of the size b2_bn_reduce_plan reports (0 otherwise, and then workspace may be null); it is scratch, ordered
+ * on `stream`, and a second small kernel folds it.  No call allocates, synchronises the host or uses atomics.
+ */
+/* ATen's launch geometry for the layer, geometry = {block.x, block.y, grid.x, grid.y}, and the workspace size in bytes. */
+int b2_bn_reduce_plan(size_t rows, size_t channels, int* geometry, size_t* workspace_bytes);
+
+/* mean, var <- the batch mean and biased variance (m2n / rows); if running_mean / running_var are given (both or neither):
+ * running <- (1 - momentum) * running + momentum * (mean, var * rows / (rows - 1)), momentum converted to float. */
+int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* mean, float* var, float* running_mean, float* running_var,
+                double momentum, void* workspace, size_t workspace_bytes, int device, void* stream);
+
+/* sum_dy <- sum(dy), sum_dy_xmu <- sum(dy * (x - mean)), grad_weight <- sum_dy_xmu * invstd, grad_bias <- sum_dy. */
+int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t channels, int dtype, const float* mean, const float* invstd,
+                          float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias, void* workspace, size_t workspace_bytes,
+                          int device, void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

@@ -40,10 +40,16 @@ GROUPS = [
 ]
 # BatchNorm kernels -> (pass, bytes per element of x moved by that pass, direction)
 BN_PASSES = [
-    ("fwd_stats", re.compile(r"batch_norm_collect_statistics"), 1, "fwd"),
+    ("fwd_stats", re.compile(r"batch_norm_collect_statistics|k_bn2d_stats\b"), 1, "fwd"),
     ("fwd_norm", re.compile(r"batch_norm_transform_input|k_bn2d_norm\b"), 2, "fwd"),
-    ("bwd_reduce", re.compile(r"batch_norm_backward_reduce"), 2, "bwd"),
+    ("bwd_reduce", re.compile(r"batch_norm_backward_reduce|k_bn2d_bwd_reduce\b"), 2, "bwd"),
     ("bwd_elemt", re.compile(r"batch_norm_backward_elemt|k_bn2d_bwd_elemt\b"), 3, "bwd"),
+]
+# The small second launch of a native reduction whose tree spans several CTA rows (it folds their partials): its time
+# belongs to the layer of the pass launched just before it
+BN_TAILS = [
+    ("fwd_stats", re.compile(r"k_bn2d_stats_merge\b")),
+    ("bwd_reduce", re.compile(r"k_bn2d_bwd_reduce_merge\b")),
 ]
 
 
@@ -128,6 +134,7 @@ def main() -> None:
     # BatchNorm kernels to layers: within each pass, occurrence k of a step is forward layer k or backward layer L-1-k
     per_shape = collections.defaultdict(lambda: collections.Counter())
     counts = collections.Counter()
+    last_layer = {}
     for _, dur, name in kernels:
         for pname, pat, _, direction in BN_PASSES:
             if pat.search(name):
@@ -135,6 +142,10 @@ def main() -> None:
                 counts[pname] += 1
                 layer = k if direction == "fwd" else L - 1 - k
                 per_shape[shapes[layer]][pname] += dur
+                last_layer[pname] = layer
+        for pname, pat in BN_TAILS:
+            if pat.search(name) and pname in last_layer:
+                per_shape[shapes[last_layer[pname]]][pname] += dur
     bn_launch_ok = all(counts[p] == S * L for p, *_ in BN_PASSES)
 
     info = card()

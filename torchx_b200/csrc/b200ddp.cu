@@ -1569,6 +1569,8 @@ namespace {
 
 constexpr int kBnFwdUnroll = 4;  // x vecs in flight per thread (forward elementwise)
 constexpr int kBnBwdUnroll = 2;  // x and dy vecs: 2 x 2 in flight per thread (backward elementwise)
+constexpr int kBnStatsUnroll = 4;   // x vecs in flight per thread (forward statistics)
+constexpr int kBnReduceUnroll = 2;  // x and dy vecs: 2 x 2 in flight per thread (backward reduce)
 
 int bn_check_shape(const char* fn, int dtype, size_t M, size_t C) {
   if (dtype != B2_DT_BFLOAT16) return fail(B2_EINVAL, "%s: dtype %d is not B2_DT_BFLOAT16", fn, dtype);
@@ -1589,6 +1591,22 @@ int bn_check_ptrs(const char* fn, std::initializer_list<BnPtr> ps) {
     if (reinterpret_cast<uintptr_t>(q.p) % q.align != 0)
       return fail(B2_EINVAL, "%s: %s is not %u-byte aligned", fn, q.name, q.align);
   }
+  return B2_OK;
+}
+
+// The reductions restate ATen's channels-last kernels, which ATen runs only for inputs with 32-bit indexing
+// (canUse32BitIndexMath: fewer than 2^31 - 1 elements); above that ATen takes another path with other bits.
+int bn_check_index32(const char* fn, size_t M, size_t C) {
+  if (M > static_cast<size_t>(INT32_MAX) / C || M * C >= static_cast<size_t>(INT32_MAX))
+    return fail(B2_EINVAL, "%s: rows*channels=%zu x %zu must be below 2^31 - 1 elements", fn, M, C);
+  return B2_OK;
+}
+
+int bn_check_workspace(const char* fn, const void* ws, size_t have, size_t need) {
+  if (need == 0) return B2_OK;
+  if (!ws) return fail(B2_EINVAL, "%s: null workspace (%zu bytes needed)", fn, need);
+  if (reinterpret_cast<uintptr_t>(ws) % 4 != 0) return fail(B2_EINVAL, "%s: workspace is not 4-byte aligned", fn);
+  if (have < need) return fail(B2_EINVAL, "%s: workspace of %zu bytes, %zu needed", fn, have, need);
   return B2_OK;
 }
 
@@ -1632,6 +1650,80 @@ int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, s
       weight, sum_dy, sum_dy_xmu, static_cast<float>(1.0 / static_cast<double>(rows)));
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+int b2_bn_reduce_plan(size_t rows, size_t channels, int* geometry, size_t* workspace_bytes) {
+  static const char* fn = "b2_bn_reduce_plan";
+  if (const int rc = bn_check_shape(fn, B2_DT_BFLOAT16, rows, channels)) return rc;
+  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
+  if (!geometry || !workspace_bytes) return fail(B2_EINVAL, "%s: null geometry or workspace_bytes", fn);
+  const bn::Tree t = bn::tree(static_cast<int>(rows), static_cast<int>(channels));
+  geometry[0] = t.block_x;
+  geometry[1] = t.block_y;
+  geometry[2] = t.grid_x;
+  geometry[3] = t.grid_y;
+  *workspace_bytes = bn::workspace_bytes(t, static_cast<int>(channels));
+  return B2_OK;
+}
+
+int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* mean, float* var, float* running_mean, float* running_var,
+                double momentum, void* workspace, size_t workspace_bytes, int device, void* stream) {
+  static const char* fn = "b2_bn_stats";
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"mean", mean, 4}, {"var", var, 4}})) return rc;
+  if ((running_mean == nullptr) != (running_var == nullptr))
+    return fail(B2_EINVAL, "%s: running_mean and running_var must both be given or both be null", fn);
+  if (running_mean)
+    if (const int rc = bn_check_ptrs(fn, {{"running_mean", running_mean, 4}, {"running_var", running_var, 4}})) return rc;
+  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
+  const bn::Tree t = bn::tree(M, C);
+  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // ATen's update lambda takes momentum as float and bessel = N / (N - 1) computed in double, rounded to float
+  const float mom = static_cast<float>(momentum);
+  const float bessel = static_cast<float>(static_cast<double>(rows) / static_cast<double>(rows - 1));
+  float* ws = static_cast<float*>(workspace);
+  const int vw = bn::reduce_vecs(t, C);
+  k_bn2d_stats<kBnStatsUnroll><<<dim3((C / 8 + vw - 1) / vw, t.grid_y), vw * t.block_y * bn::kAtenLoads, 0, s>>>(
+      static_cast<const uint16_t*>(x), M, C, t, vw, mean, var, running_mean, running_var, mom, bessel, ws);
+  if (t.grid_y > 1) {
+    const int mw = bn::merge_vecs(t, C);
+    k_bn2d_stats_merge<<<(C / 8 + mw - 1) / mw, mw * t.block_y, 0, s>>>(C, t, mw, ws, mean, var, running_mean, running_var, mom, bessel);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm statistics kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t channels, int dtype, const float* mean, const float* invstd,
+                          float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias, void* workspace, size_t workspace_bytes,
+                          int device, void* stream) {
+  static const char* fn = "b2_bn_backward_reduce";
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}, {"mean", mean, 4}, {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4},
+                                        {"sum_dy_xmu", sum_dy_xmu, 4}, {"grad_weight", grad_weight, 4}, {"grad_bias", grad_bias, 4}}))
+    return rc;
+  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
+  const bn::Tree t = bn::tree(M, C);
+  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* ws = static_cast<float*>(workspace);
+  const int vw = bn::reduce_vecs(t, C);
+  k_bn2d_bwd_reduce<kBnReduceUnroll><<<dim3((C / 8 + vw - 1) / vw, t.grid_y), vw * t.block_y * bn::kAtenLoads, 0, s>>>(
+      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), M, C, t, vw, mean, invstd, sum_dy, sum_dy_xmu, grad_weight,
+      grad_bias, ws);
+  if (t.grid_y > 1) {
+    const int mw = bn::merge_vecs(t, C);
+    k_bn2d_bwd_reduce_merge<<<(C / 8 + mw - 1) / mw, mw * t.block_y, 0, s>>>(C, t, mw, ws, invstd, sum_dy, sum_dy_xmu, grad_weight,
+                                                                             grad_bias);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward reduce kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 

@@ -1,16 +1,18 @@
-// b2_bn.cuh — the elementwise passes of training-mode BatchNorm2d on channels-last bf16 activations
-// (b2_bn_forward_elemt / b2_bn_backward_elemt).
+// b2_bn.cuh — training-mode BatchNorm2d on channels-last bf16 activations: the two reductions (b2_bn_stats /
+// b2_bn_backward_reduce) and the two elementwise passes (b2_bn_forward_elemt / b2_bn_backward_elemt).
 //
 // The data is the row-major [M, C] view of an NHWC-contiguous tensor (M = N*H*W).  Each thread owns one 16-byte vec of
-// 8 channels and walks rows; a CTA covers a tile of `cw` vecs x `rows` rows per trip and U trips' loads are issued
-// before any is used.
-//   k_bn2d_norm       read x, write y       invstd = rsqrt(var + eps), y = w * (x - mean) * invstd + b
-//   k_bn2d_bwd_elemt  read x, dy, write dx  dx = (dy - sum_dy/M - (x - mean) * invstd^2 * sum_dy_xmu/M) * invstd * w
-// Their inputs are ATen's own reductions (batch_norm_update_stats' mean / var, batch_norm_backward_reduce's sums) and their
-// arithmetic is that of ATen's batch_norm_update_stats_and_invert, batch_norm_transform_input_channels_last_kernel and
-// batch_norm_backward_elemt_channels_last_kernel, expression for expression: y, invstd and dx are ATen's bits.
-// Both passes walk their row blocks last one first: the reduction before them streams the rows upwards, so a layer that
-// fits in L2 starts on the rows it read last.
+// 8 channels and walks rows.
+//   k_bn2d_stats       read x                mean, var = m2n / M, running statistics (ATen's Welford tree, below)
+//   k_bn2d_bwd_reduce  read x, dy            sum_dy, sum_dy_xmu, grad_weight = sum_dy_xmu * invstd, grad_bias = sum_dy
+//   k_bn2d_norm        read x, write y       invstd = rsqrt(var + eps), y = w * (x - mean) * invstd + b
+//   k_bn2d_bwd_elemt   read x, dy, write dx  dx = (dy - sum_dy/M - (x - mean) * invstd^2 * sum_dy_xmu/M) * invstd * w
+// The arithmetic is that of ATen's batch_norm_collect_statistics_channels_last_kernel, batch_norm_update_stats(_and_invert),
+// batch_norm_backward_reduce_channels_last_kernel, batch_norm_transform_input_channels_last_kernel and
+// batch_norm_backward_elemt_channels_last_kernel, expression for expression and, for the reductions, in ATen's order:
+// every output is ATen's bits (DESIGN.md 2.4).
+// The reductions walk the rows upwards and the elementwise passes walk their row blocks last one first, so a layer that
+// fits in L2 starts on the rows the reduction read last.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -84,6 +86,178 @@ __device__ __forceinline__ Lane lane(const Plan& p, unsigned long long C) {
   l.col = (static_cast<unsigned long long>(blockIdx.x) * p.cw + t % p.cw) * 8;
   l.on = l.r < p.rows && l.col < C;
   return l;
+}
+
+// ---- ATen's reduction tree ------------------------------------------------------------------------------------------------
+// ATen's channels-last reductions launch flexible_launch_configs(M, C, block, grid, coop = true) with 4 parallel loads per
+// thread.  A channel's result depends only on block.y and grid.y: thread (ty, by) with slot j runs one sequential chain over
+// rows by*block_y + ty + (4i + j)*S, S = block_y*grid_y, i < loops; the 4 slots merge in order, then the block_y threads
+// of a CTA pairwise by halving offsets, then (grid_y > 1) the CTA partials in ATen's last-block order.  block.x only decides
+// which channels share a CTA.  Every quantity here is a function of the shape alone (no device query), and M*C < 2^31.
+constexpr int kAtenMaxBlock = 512;      // MAX_BLOCK_SIZE
+constexpr int kAtenTileW = 32;          // OPTIMAL_TILE_W
+constexpr int kAtenElemsPerThread = 16; // ELEMENTS_PER_THREAD
+constexpr int kAtenMaxHBlock = 128;     // MAX_H_BLOCK
+constexpr int kAtenLoads = 4;           // ELEMENTS_PER_ITER, the kernels' PARALLEL_LOADS
+
+struct Tree {
+  int block_x, block_y, grid_x, grid_y;  // ATen's launch
+  int seq;    // S = block_y * grid_y
+  int loops;  // loop_count: rows per chain, the same for every chain
+};
+
+inline int last_pow2(unsigned n) {
+  n |= n >> 1;
+  n |= n >> 2;
+  n |= n >> 4;
+  n |= n >> 8;
+  n |= n >> 16;
+  const int p = static_cast<int>(n - (n >> 1));
+  return p > 1 ? p : 1;
+}
+
+inline Tree tree(int M, int C) {
+  Tree t;
+  const int lp = last_pow2(static_cast<unsigned>(C));
+  t.block_x = lp < kAtenTileW ? lp : kAtenTileW;
+  const int by = last_pow2(static_cast<unsigned>((M + kAtenElemsPerThread - 1) / kAtenElemsPerThread));
+  t.block_y = by < kAtenMaxBlock / t.block_x ? by : kAtenMaxBlock / t.block_x;
+  if (t.block_x * t.block_y != kAtenMaxBlock) t.block_x = lp < kAtenMaxBlock / t.block_y ? lp : kAtenMaxBlock / t.block_y;
+  t.grid_x = (C + t.block_x - 1) / t.block_x;
+  const int gy = (M + t.block_y * kAtenElemsPerThread - 1) / (t.block_y * kAtenElemsPerThread);
+  t.grid_y = gy < kAtenMaxHBlock ? gy : kAtenMaxHBlock;
+  if (t.grid_y < 8) t.grid_y = 1;  // coop_flag
+  t.seq = t.block_y * t.grid_y;
+  t.loops = 1 + (M - 1) / (t.seq * kAtenLoads);
+  return t;
+}
+
+// Our CTA: `vw` vecs x block_y x the 4 slots, one chain of 8 channels per thread (vec fastest, so a warp reads whole
+// rows); one CTA row per ATen CTA row (blockIdx.y = by).  block_y <= 512 / 8, so a CTA has at most 256 threads.
+inline int reduce_vecs(const Tree& t, int C) {
+  const int per = t.block_y * kAtenLoads;
+  const int vw = kBnThreads / per > 1 ? kBnThreads / per : 1;
+  return vw < C / 8 ? vw : C / 8;
+}
+// The grid_y merge: `vw` vecs x block_y threads per CTA.
+inline int merge_vecs(const Tree& t, int C) {
+  const int vw = kBnThreads / t.block_y > 1 ? kBnThreads / t.block_y : 1;
+  return vw < C / 8 ? vw : C / 8;
+}
+// Partials of the grid_y merge, float [by][C] mean (sum_dy) and m2n (sum_dy_xmu) and, for the statistics, int [by][C/8]
+// counts: ATen's staging, 3 words per (channel, by) there.
+inline size_t workspace_bytes(const Tree& t, int C) {
+  return t.grid_y > 1 ? static_cast<size_t>(t.grid_y) * (2 * static_cast<size_t>(C) + C / 8) * 4 : 0;
+}
+
+// Welford state of one chain over 8 channels (the count is the same for all 8: rows are valid for a whole vec or not at all).
+struct Welford {
+  int n;
+  float mean[8], m2n[8];
+};
+
+// ATen's welford_merge_element, in the two contractions its build uses (sm_90 SASS, DESIGN.md 2.4): merging the 4 slots
+// inside a thread fuses mean_new * count_new (FFMA mean_new, cn, mean * c), every other merge fuses mean * count.  A
+// zero-count merge is not skipped: (mean * c) * (1 / max(1, c)) can change bits, as in ATen.
+template <bool kSlots>
+__device__ __forceinline__ void welford_merge(Welford& a, int cn, const float (&mn)[8], const float (&m2)[8]) {
+  const int tot = a.n + cn;
+  const float factor = __frcp_rn(__int2float_rn(tot > 1 ? tot : 1));
+  const float fc = __int2float_rn(a.n), fcn = __int2float_rn(cn);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float d0 = __fsub_rn(a.mean[k], mn[k]);
+    const float t = __fmul_rn(fc, __fmul_rn(fcn, __fmul_rn(d0, d0)));
+    const float s = kSlots ? __fmaf_rn(mn[k], fcn, __fmul_rn(a.mean[k], fc)) : __fmaf_rn(a.mean[k], fc, __fmul_rn(mn[k], fcn));
+    a.mean[k] = __fmul_rn(s, factor);
+    a.m2n[k] = __fadd_rn(a.m2n[k], __fmaf_rn(t, factor, m2[k]));
+  }
+  a.n = tot;
+}
+
+// Shared-memory slots of a CTA's states: [8][256] means and m2ns (sum_dy / sum_dy_xmu), [256] counts.
+struct Smem {
+  float a[8][kBnThreads];
+  float b[8][kBnThreads];
+  int n[kBnThreads];
+};
+
+__device__ __forceinline__ void put(Smem& s, int slot, const Welford& w) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    s.a[k][slot] = w.mean[k];
+    s.b[k][slot] = w.m2n[k];
+  }
+  s.n[slot] = w.n;
+}
+
+template <bool kSlots>
+__device__ __forceinline__ void merge_from(Welford& w, const Smem& s, int slot) {
+  float mn[8], m2[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    mn[k] = s.a[k][slot];
+    m2[k] = s.b[k][slot];
+  }
+  welford_merge<kSlots>(w, s.n[slot], mn, m2);
+}
+
+__device__ __forceinline__ void put(Smem& s, int slot, const float (&a)[8], const float (&b)[8]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    s.a[k][slot] = a[k];
+    s.b[k][slot] = b[k];
+  }
+}
+
+__device__ __forceinline__ void add_from(float (&a)[8], float (&b)[8], const Smem& s, int slot) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    a[k] = __fadd_rn(a[k], s.a[k][slot]);
+    b[k] = __fadd_rn(b[k], s.b[k][slot]);
+  }
+}
+
+// ATen's welford_merge_block_vertical / merge_block_vertical_backward over ty (slot = v + vw * ty): ty < off takes ty + off
+// for off = block_y/2 .. 1.  Every thread of the CTA calls it; `live` threads hold a state.
+template <class Merge>
+__device__ __forceinline__ void vertical(int v, int vw, int ty, int block_y, bool live, Merge&& merge) {
+  for (int off = block_y / 2; off > 0; off >>= 1) {
+    __syncthreads();
+    if (live && ty < off) merge(v + vw * (ty + off), v + vw * ty);
+  }
+}
+
+// The end of ATen's statistics kernel and of batch_norm_update_stats_and_invert's running-statistics lambda (fp32:
+// 1 - momentum by FADD, FMUL (1 - momentum) * running, FFMA x, momentum, that; bessel = M / (M - 1) in double rounded to
+// float at the launch).
+__device__ __forceinline__ void stats_out(const Welford& w, unsigned long long col, float* __restrict__ mean, float* __restrict__ var,
+                                          float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel) {
+  const float omm = __fsub_rn(1.0f, momentum);
+  const float fn = __int2float_rn(w.n);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float v = __fdiv_rn(w.m2n[k], fn);
+    mean[col + k] = w.mean[k];
+    var[col + k] = v;
+    if (running_mean != nullptr) {
+      running_mean[col + k] = __fmaf_rn(w.mean[k], momentum, __fmul_rn(omm, running_mean[col + k]));
+      running_var[col + k] = __fmaf_rn(__fmul_rn(v, bessel), momentum, __fmul_rn(omm, running_var[col + k]));
+    }
+  }
+}
+
+// The end of ATen's backward reduce: grad_weight = sum_dy_xmu * invstd (FMUL), grad_bias = sum_dy.
+__device__ __forceinline__ void reduce_out(const float (&sdy)[8], const float (&sxmu)[8], unsigned long long col, const float* __restrict__ invstd,
+                                           float* __restrict__ sum_dy, float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight,
+                                           float* __restrict__ grad_bias) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    sum_dy[col + k] = sdy[k];
+    sum_dy_xmu[col + k] = sxmu[k];
+    grad_weight[col + k] = __fmul_rn(sxmu[k], invstd[col + k]);
+    grad_bias[col + k] = sdy[k];
+  }
 }
 
 }  // namespace bn
@@ -183,4 +357,231 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
       }
     }
   }
+}
+
+// ---- forward statistics -------------------------------------------------------------------------------------------------
+// One thread per (vec, ty, j) of ATen CTA row by = blockIdx.y: the chain's Welford update per row in ATen's contraction
+// (delta0 = x - mean; mean = FFMA delta0, 1/count, mean; delta1 = x - mean; m2n = FFMA delta0*delta1, is_valid, m2n), one
+// IEEE reciprocal of the count per row for all 8 channels.  A slot past M still runs the update with x = 0, 1/count = 0,
+// is_valid = 0, as ATen's does: that is not a no-op once the mean is inf or NaN.  U rows' loads are issued before the
+// first is used.  Then the slot merge and the vertical merge through shared memory; with grid_y == 1 the CTA writes the
+// outputs, otherwise its partial, which k_bn2d_stats_merge folds in ATen's last-block order.
+template <int U>
+__global__ void __launch_bounds__(bn::kBnThreads)
+    k_bn2d_stats(const uint16_t* __restrict__ x, int M, int C, bn::Tree t, int vw, float* __restrict__ mean, float* __restrict__ var,
+                 float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel, float* __restrict__ ws) {
+  using namespace bn;
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  Welford w;
+  w.n = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) w.mean[k] = w.m2n[k] = 0.0f;
+  if (on) {
+    const int stride = kAtenLoads * t.seq;
+    int row = blockIdx.y * t.block_y + ty + j * t.seq;
+    for (int i = 0; i < t.loops; i += U) {
+      uint4 q[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int r = row + u * stride;
+        q[u] = i + u < t.loops && r < M ? ld_vec(x + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (i + u < t.loops) {
+          float inv = 0.0f, valid = 0.0f;
+          if (row + u * stride < M) {
+            ++w.n;
+            inv = __frcp_rn(__int2float_rn(w.n));
+            valid = 1.0f;
+          }
+          float f[8];
+          unpack(q[u], f);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const float d0 = __fsub_rn(f[k], w.mean[k]);
+            w.mean[k] = __fmaf_rn(d0, inv, w.mean[k]);
+            const float d1 = __fsub_rn(f[k], w.mean[k]);
+            w.m2n[k] = __fmaf_rn(__fmul_rn(d0, d1), valid, w.m2n[k]);
+          }
+        }
+      }
+      row += U * stride;
+    }
+  }
+  put(sm, v + vw * (ty + t.block_y * j), w);
+  __syncthreads();
+  const bool lead = on && j == 0;
+  if (lead) {
+#pragma unroll
+    for (int jj = 1; jj < kAtenLoads; ++jj) merge_from<true>(w, sm, v + vw * (ty + t.block_y * jj));
+    put(sm, v + vw * ty, w);
+  }
+  vertical(v, vw, ty, t.block_y, lead, [&](int src, int dst) {
+    merge_from<false>(w, sm, src);
+    put(sm, dst, w);
+  });
+  if (!lead || ty != 0) return;
+  if (t.grid_y == 1) {
+    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
+    return;
+  }
+  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    ws[base + k] = w.mean[k];
+    ws[static_cast<size_t>(t.grid_y) * C + base + k] = w.m2n[k];
+  }
+  reinterpret_cast<int*>(ws + 2 * static_cast<size_t>(t.grid_y) * C)[static_cast<size_t>(blockIdx.y) * (C / 8) + vec] = w.n;
+}
+
+// ATen's last block: thread ty merges partials y = ty, ty + block_y, ... into a zero state, then the vertical merge.
+__global__ void __launch_bounds__(bn::kBnThreads)
+    k_bn2d_stats_merge(int C, bn::Tree t, int vw, const float* __restrict__ ws, float* __restrict__ mean, float* __restrict__ var,
+                       float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel) {
+  using namespace bn;
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = tid / vw;
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  const int* cnt = reinterpret_cast<const int*>(ws + 2 * static_cast<size_t>(t.grid_y) * C);
+  Welford w;
+  w.n = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) w.mean[k] = w.m2n[k] = 0.0f;
+  if (on) {
+    for (int y = ty; y < t.grid_y; y += t.block_y) {
+      const size_t base = static_cast<size_t>(y) * C + col;
+      float mn[8], m2[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        mn[k] = ws[base + k];
+        m2[k] = ws[static_cast<size_t>(t.grid_y) * C + base + k];
+      }
+      welford_merge<false>(w, cnt[static_cast<size_t>(y) * (C / 8) + vec], mn, m2);
+    }
+    put(sm, v + vw * ty, w);
+  }
+  vertical(v, vw, ty, t.block_y, on, [&](int src, int dst) {
+    merge_from<false>(w, sm, src);
+    put(sm, dst, w);
+  });
+  if (on && ty == 0) stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
+}
+
+// ---- backward reduce ----------------------------------------------------------------------------------------------------
+// The same chains with plain sums: sum_dy += dy (FADD), sum_dy_xmu = FFMA (x - mean), dy, sum_dy_xmu; a slot past M adds
+// dy = 0 and 0 * (0 - mean).  ATen's kernel returns early from threads with c_offset >= C or m_offset >= M: the first only
+// ever holds channels no valid thread reads (the vertical merge pairs threads of one threadIdx.x), and m_offset =
+// by*block_y + ty < block_y*grid_y <= M for every geometry flexible_launch_configs makes, so no valid channel is affected.
+template <int U>
+__global__ void __launch_bounds__(bn::kBnThreads)
+    k_bn2d_bwd_reduce(const uint16_t* __restrict__ dy, const uint16_t* __restrict__ x, int M, int C, bn::Tree t, int vw,
+                      const float* __restrict__ mean, const float* __restrict__ invstd, float* __restrict__ sum_dy,
+                      float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight, float* __restrict__ grad_bias,
+                      float* __restrict__ ws) {
+  using namespace bn;
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  float sdy[8], sxmu[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sdy[k] = sxmu[k] = 0.0f;
+  if (on) {
+    float m[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) m[k] = mean[col + k];
+    const int stride = kAtenLoads * t.seq;
+    int row = blockIdx.y * t.block_y + ty + j * t.seq;
+    for (int i = 0; i < t.loops; i += U) {
+      uint4 qd[U], qx[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int r = row + u * stride;
+        const bool ld = i + u < t.loops && r < M;
+        qd[u] = ld ? ld_vec(dy + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+        qx[u] = ld ? ld_vec(x + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (i + u < t.loops) {
+          float fd[8], fx[8];
+          unpack(qd[u], fd);
+          unpack(qx[u], fx);
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            sdy[k] = __fadd_rn(sdy[k], fd[k]);
+            sxmu[k] = __fmaf_rn(__fsub_rn(fx[k], m[k]), fd[k], sxmu[k]);
+          }
+        }
+      }
+      row += U * stride;
+    }
+  }
+  put(sm, v + vw * (ty + t.block_y * j), sdy, sxmu);
+  __syncthreads();
+  const bool lead = on && j == 0;
+  if (lead) {
+#pragma unroll
+    for (int jj = 1; jj < kAtenLoads; ++jj) add_from(sdy, sxmu, sm, v + vw * (ty + t.block_y * jj));
+    put(sm, v + vw * ty, sdy, sxmu);
+  }
+  vertical(v, vw, ty, t.block_y, lead, [&](int src, int dst) {
+    add_from(sdy, sxmu, sm, src);
+    put(sm, dst, sdy, sxmu);
+  });
+  if (!lead || ty != 0) return;
+  if (t.grid_y == 1) {
+    reduce_out(sdy, sxmu, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
+    return;
+  }
+  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    ws[base + k] = sdy[k];
+    ws[static_cast<size_t>(t.grid_y) * C + base + k] = sxmu[k];
+  }
+}
+
+// ATen's last block for the sums: from 0, add partials y = ty, ty + block_y, ..., then the vertical merge.
+__global__ void __launch_bounds__(bn::kBnThreads)
+    k_bn2d_bwd_reduce_merge(int C, bn::Tree t, int vw, const float* __restrict__ ws, const float* __restrict__ invstd,
+                            float* __restrict__ sum_dy, float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight,
+                            float* __restrict__ grad_bias) {
+  using namespace bn;
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = tid / vw;
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  float sdy[8], sxmu[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sdy[k] = sxmu[k] = 0.0f;
+  if (on) {
+    for (int y = ty; y < t.grid_y; y += t.block_y) {
+      const size_t base = static_cast<size_t>(y) * C + col;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        sdy[k] = __fadd_rn(sdy[k], ws[base + k]);
+        sxmu[k] = __fadd_rn(sxmu[k], ws[static_cast<size_t>(t.grid_y) * C + base + k]);
+      }
+    }
+    put(sm, v + vw * ty, sdy, sxmu);
+  }
+  vertical(v, vw, ty, t.block_y, on, [&](int src, int dst) {
+    add_from(sdy, sxmu, sm, src);
+    put(sm, dst, sdy, sxmu);
+  });
+  if (on && ty == 0) reduce_out(sdy, sxmu, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
 }

@@ -99,6 +99,9 @@ SYMBOLS = [
     "b2_batchnorm_stats",
     "b2_bn_forward_elemt",
     "b2_bn_backward_elemt",
+    "b2_bn_reduce_plan",
+    "b2_bn_stats",
+    "b2_bn_backward_reduce",
     "b2_barrier",
     "b2_local_pass",
 ]
@@ -228,6 +231,12 @@ def lib() -> ctypes.CDLL:
     L.b2_bn_forward_elemt.argtypes = [vp, vp, sz, sz, i, vp, vp, vp, vp, ctypes.c_double, vp, i, vp]
     L.b2_bn_backward_elemt.restype = i
     L.b2_bn_backward_elemt.argtypes = [vp, vp, vp, sz, sz, i, vp, vp, vp, vp, vp, i, vp]
+    L.b2_bn_reduce_plan.restype = i
+    L.b2_bn_reduce_plan.argtypes = [sz, sz, ctypes.POINTER(i), ctypes.POINTER(sz)]
+    L.b2_bn_stats.restype = i
+    L.b2_bn_stats.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, ctypes.c_double, vp, sz, i, vp]
+    L.b2_bn_backward_reduce.restype = i
+    L.b2_bn_backward_reduce.argtypes = [vp, vp, sz, sz, i, vp, vp, vp, vp, vp, vp, vp, sz, i, vp]
     L.b2_barrier.restype = i
     L.b2_barrier.argtypes = [vp, vp]
     L.b2_local_pass.restype = i

@@ -1,12 +1,13 @@
-"""Training-mode ``BatchNorm2d`` with native sm_90a elementwise passes for channels-last bf16 activations.
+"""Training-mode ``BatchNorm2d`` on native sm_90a kernels for channels-last bf16 activations.
 
-ATen's channels-last BatchNorm kernels give each thread one channel and load one 2-byte element at a time.  The two
-elementwise passes, the forward normalise and the backward ``dx``, move the most bytes (4 and 6 per element); here they
-read and write 16-byte vecs of 8 channels (``b2_bn_forward_elemt`` / ``b2_bn_backward_elemt``, DESIGN.md 2.3).  The
-reductions stay ATen's own (``torch.batch_norm_update_stats``, ``torch.batch_norm_backward_reduce``) and the elementwise
-arithmetic is ATen's expression for expression, so every output, gradient and running statistic is the bits
-``nn.BatchNorm2d`` computes (DESIGN.md 2.4).  fp16 activations stay on ATen: there torch's BatchNorm runs cuDNN's kernels,
-whose bits these passes do not reproduce.
+ATen's channels-last BatchNorm kernels give each thread one channel and load one 2-byte element at a time.  Here all four
+passes read (and write) 16-byte vecs of 8 channels (DESIGN.md 2.3): the forward statistics and the backward reduce
+(``b2_bn_stats`` / ``b2_bn_backward_reduce``), which run ATen's reduction tree in ATen's order, and the forward normalise
+and backward ``dx`` (``b2_bn_forward_elemt`` / ``b2_bn_backward_elemt``), ATen's expressions.  So every output, gradient
+and running statistic is the bits ``nn.BatchNorm2d`` computes (DESIGN.md 2.4).  An input of 2^31 - 1 elements or more keeps
+ATen's reduction calls (``torch.batch_norm_update_stats``, ``torch.batch_norm_backward_reduce``), as ATen reduces those on
+another path.  fp16 activations stay on ATen: there torch's BatchNorm runs cuDNN's kernels, whose bits these passes do not
+reproduce.
 
 ``BatchNorm2d`` is ``nn.BatchNorm2d`` with the same parameters, buffers, state-dict keys and hooks; it takes the native
 path only for an input that the kernels cover exactly (``native_eligible``) and calls ``nn.BatchNorm2d.forward``
@@ -14,6 +15,8 @@ unchanged for everything else: eval mode, fp32 or NCHW inputs, CPU tensors, non-
 rejects.  ``convert_batchnorm`` switches the layers of a model over in place.
 """
 from __future__ import annotations
+
+import ctypes
 
 import torch
 from torch import nn
@@ -24,20 +27,29 @@ from torchx_b200.ddp import _native as N
 
 
 class _NativeBatchNorm(torch.autograd.Function):
-    """Training-mode batch norm of a channels-last [N, C, H, W] bf16 tensor: ATen's ``native_batch_norm`` with the
-    two elementwise passes native.  Saves what ATen saves: the input, the weight and the batch mean / invstd."""
+    """Training-mode batch norm of a channels-last [N, C, H, W] bf16 tensor: ATen's ``native_batch_norm`` with its
+    passes native.  Saves what ATen saves: the input, the weight and the batch mean / invstd."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps):
         n, c, h, w = x.shape
         dev = x.device
-        # ATen's training forward: batch_norm_mean_var, then the running-statistics update (the same kernels as here)
-        mean, var = torch.batch_norm_update_stats(x, running_mean, running_var, momentum)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        # ATen's training forward: batch_norm_mean_var, then the running-statistics update
+        if native_reductions(x):
+            mean = torch.empty(c, dtype=torch.float32, device=dev)
+            var = torch.empty(c, dtype=torch.float32, device=dev)
+            ws, ws_bytes = _workspace(n * h * w, c, dev)
+            N.check(N.lib().b2_bn_stats(x.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16, mean.data_ptr(), var.data_ptr(),
+                                        _ptr(running_mean), _ptr(running_var), float(momentum), _ptr(ws), ws_bytes, dev.index,
+                                        stream))
+        else:
+            mean, var = torch.batch_norm_update_stats(x, running_mean, running_var, momentum)
         y = torch.empty_like(x, memory_format=torch.channels_last)
         invstd = torch.empty(c, dtype=torch.float32, device=dev)
         N.check(N.lib().b2_bn_forward_elemt(x.data_ptr(), y.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16, weight.data_ptr(),
                                             bias.data_ptr(), mean.data_ptr(), var.data_ptr(), float(eps), invstd.data_ptr(),
-                                            dev.index, torch.cuda.current_stream(dev).cuda_stream))
+                                            dev.index, stream))
         ctx.save_for_backward(x, weight, mean, invstd)
         return y
 
@@ -49,15 +61,48 @@ class _NativeBatchNorm(torch.autograd.Function):
         if not (need_x or need_w or need_b):
             return None, None, None, None, None, None, None
         dy = grad_output.contiguous(memory_format=torch.channels_last)
-        sum_dy, sum_dy_xmu, gw, gb = torch.batch_norm_backward_reduce(dy, x, mean, invstd, weight, need_x, need_w, need_b)
+        n, c, h, w = x.shape
+        dev = x.device
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if native_reductions(x):
+            sum_dy, sum_dy_xmu, gw, gb = (torch.empty(c, dtype=torch.float32, device=dev) for _ in range(4))
+            ws, ws_bytes = _workspace(n * h * w, c, dev)
+            N.check(N.lib().b2_bn_backward_reduce(dy.data_ptr(), x.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16, mean.data_ptr(),
+                                                  invstd.data_ptr(), sum_dy.data_ptr(), sum_dy_xmu.data_ptr(), gw.data_ptr(),
+                                                  gb.data_ptr(), _ptr(ws), ws_bytes, dev.index, stream))
+        else:
+            sum_dy, sum_dy_xmu, gw, gb = torch.batch_norm_backward_reduce(dy, x, mean, invstd, weight, need_x, need_w, need_b)
         dx = None
         if need_x:
-            n, c, h, w = x.shape
             dx = torch.empty_like(x, memory_format=torch.channels_last)
             N.check(N.lib().b2_bn_backward_elemt(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16,
                                                  weight.data_ptr(), mean.data_ptr(), invstd.data_ptr(), sum_dy.data_ptr(),
-                                                 sum_dy_xmu.data_ptr(), x.device.index, torch.cuda.current_stream(x.device).cuda_stream))
+                                                 sum_dy_xmu.data_ptr(), dev.index, stream))
         return dx, gw if need_w else None, gb if need_b else None, None, None, None, None
+
+
+# ATen reduces with its channels-last kernels only under 32-bit indexing (canUse32BitIndexMath: fewer than 2^31 - 1
+# elements); above that it takes its general path, whose bits the native reductions do not restate.
+_INDEX32_LIMIT = 2**31 - 1
+
+
+def native_reductions(x: torch.Tensor) -> bool:
+    """True when the two reductions of an eligible input run natively (``b2_bn_stats`` / ``b2_bn_backward_reduce``): where
+    ATen itself would run its channels-last kernels.  Larger inputs keep ATen's own reduction calls."""
+    return x.numel() < _INDEX32_LIMIT
+
+
+def _ptr(t) -> int:
+    return 0 if t is None else t.data_ptr()
+
+
+def _workspace(rows: int, channels: int, dev: torch.device):
+    """Scratch for the reductions' grid_y merge, from torch's caching allocator (stream-ordered), or None."""
+    geom, nbytes = (ctypes.c_int * 4)(), ctypes.c_size_t()
+    N.check(N.lib().b2_bn_reduce_plan(rows, channels, geom, ctypes.byref(nbytes)))
+    if nbytes.value == 0:
+        return None, 0
+    return torch.empty(nbytes.value // 4, dtype=torch.float32, device=dev), nbytes.value
 
 
 def native_eligible(bn: nn.BatchNorm2d, x: torch.Tensor) -> bool:
