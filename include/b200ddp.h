@@ -20,6 +20,7 @@
  *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
  *   b2_reduce_scatter  <- `dist.reduce_scatter_tensor` / `dist.reduce_scatter`
  *   b2_alltoall, b2_alltoall_max_bytes <- `dist.all_to_all_single` / `dist.all_to_all`
+ *   b2_p2p             <- dist.send / dist.recv / dist.batch_isend_irecv (and the gather / scatter built on them)
  *   b2_batchnorm_stats <- torch's SyncBatchNorm forward: all_gather of (mean, invstd, count) + the count mask +
  *                         batch_norm_gather_stats_with_counts (torch/nn/modules/_functions.py)
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
@@ -33,8 +34,10 @@
  * is enqueued asynchronously on the caller's CUDA stream (`stream` is a cudaStream_t
  * passed as void*; NULL = the legacy default stream).  A communicator is a single
  * stream-ordered sequence of collectives (like an NCCL communicator): all ranks must
- * issue the same operations in the same order, and calls on one communicator must not
- * be issued concurrently from several host threads.
+ * issue the same collectives in the same order, and calls on one communicator must not
+ * be issued concurrently from several host threads.  Point-to-point calls (b2_p2p) involve
+ * only the ranks they name; those of one communicator must be issued on one stream, or on
+ * streams ordered against each other, because its channel counters are per-communicator state.
  */
 #ifndef B200DDP_H_
 #define B200DDP_H_
@@ -111,7 +114,9 @@ const char* b2_last_error(void);
  * counter: a re-launched gang uses a new epoch so survivors never map a dead peer's memory).
  * `device` is the CUDA ordinal this rank is pinned to.  `stage_bytes` is the per-rank size of ONE
  * of the two symmetric staging buffers (0 = default 512 MiB); messages larger than what fits are
- * chunked internally.  `timeout_ms` bounds the rendezvous (0 = default 120 s).
+ * chunked internally.  `timeout_ms` bounds the rendezvous (0 = default 120 s).  The collectives of a
+ * communicator are issued by all ranks in the same order; its point-to-point calls (b2_p2p) on one stream,
+ * or on streams ordered against each other.
  */
 int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char* shm_name,
                    uint64_t epoch, size_t stage_bytes, int timeout_ms);
@@ -164,7 +169,8 @@ int b2_comm_set_param(b2_comm_t* comm, const char* name, long long value);
 /*
  * Non-blocking health check: B2_OK, B2_ETIMEOUT if any kernel of this communicator gave up
  * waiting for a peer (its output is then undefined), or B2_EINVAL if an all-to-all's split sizes
- * disagreed across ranks or exceeded the per-pair limit (see b2_alltoall).  Reads a host-mapped
+ * disagreed across ranks or exceeded the per-pair limit (see b2_alltoall), or a point-to-point
+ * receive's byte count disagreed with its sender's (see b2_p2p).  Reads a host-mapped
  * status word; does not synchronise the device.  Either code poisons the communicator: every later
  * collective returns B2_ESTATE.
  */
@@ -351,6 +357,45 @@ int b2_alltoall(b2_comm_t* comm, void* const* out, const size_t* recv_bytes, con
 /* The most bytes one rank may send another in one b2_alltoall: a stage region less its 16-byte count header (the stage
  * size is b2_comm_create's stage_bytes, default 512 MiB, divided into W + 1 regions).  0 for a null communicator. */
 size_t b2_alltoall_max_bytes(const b2_comm_t* comm);
+
+/*
+ * Point-to-point: a batch of 1..B2_P2P_MAX_OPS sends and receives, a bit-exact copy of bytes (any dtype), in ONE launch.
+ * `ops` is a HOST array copied into the kernel parameters by the call.  A send gives `bytes` bytes at `ptr` to rank
+ * `peer`; a receive writes into `ptr` the next message rank `peer` sends this rank, which must have exactly `bytes` bytes.
+ * Messages between an ordered pair of ranks (a channel) match in issue order, as NCCL's do; a batch may hold several ops
+ * on one channel (they run in list order) and ops on any other channels, and it never waits on itself: ops of one batch
+ * make progress whatever their order in the list and in the peer's batch.  send / recv / isend / irecv are batches of one.
+ *   - A null communicator or op list, n_ops outside 1..B2_P2P_MAX_OPS, a peer out of range or equal to this rank (which
+ *     rules out W == 1), a null pointer with a non-zero byte count, or a receive range that overlaps any other range of the
+ *     batch: B2_EINVAL before anything is launched; a poisoned communicator: B2_ESTATE.
+ *   - Every wait is bounded: a kernel that gives up records B2_ETIMEOUT for b2_comm_status.  Once a wait of this
+ *     communicator has given up, or a receive has found a size mismatch, its other waits give up within a few polls
+ *     instead of a timeout each.  A chunk whose wait gave up is neither written nor handed on, so a receiver that arrives
+ *     after its sender gave up waits for it and records its own timeout rather than taking stale bytes.
+ *   - A receive whose byte count is not the sender's: the receiver writes none of that message and records B2_EINVAL,
+ *     which poisons only its own communicator.  A sender whose message is at most b2_p2p_eager_bytes has already
+ *     finished; a larger one waits for the slots the receiver never hands back until its timeout.  A receiver that
+ *     expects more chunks than its sender sent stops waiting for the missing ones once it has recorded the mismatch.
+ *   - Deadlocks the caller can create: two ranks that each send more than b2_p2p_eager_bytes before their recv, in
+ *     separate calls, wait until the timeout, exactly as with NCCL outside a group; the cure is one batch.  The same holds
+ *     for a point-to-point call ordered on one rank against a collective that the peer issues in the opposite order.
+ * Point-to-point uses its own buffers and counters and never touches the collectives' state, so a collective's result and
+ * protocol are the same whatever point-to-point traffic runs before, after or between collectives.
+ */
+#define B2_P2P_MAX_OPS 64
+typedef struct b2_p2p_op {
+  int peer;    /* the other rank */
+  int is_send; /* nonzero: send, 0: receive */
+  void* ptr;   /* device pointer of this rank (may be NULL when bytes == 0) */
+  size_t bytes;
+} b2_p2p_op_t;
+
+int b2_p2p(b2_comm_t* comm, const b2_p2p_op_t* ops, int n_ops, void* stream);
+
+/* The largest message a send completes without the matching receive having been launched, once the earlier messages on
+ * its channel have been received: the inbox of K slots of one chunk each, less their 16-byte headers (8 x 512 KiB - 128
+ * bytes).  0 for a null communicator. */
+size_t b2_p2p_eager_bytes(const b2_comm_t* comm);
 
 /*
  * SyncBatchNorm statistics: in place, mean[c] / invstd[c] <- the merge of every rank's (mean, invstd, count) over the ranks

@@ -17,6 +17,7 @@
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
 //   * reduce-scatter with the allreduce's arithmetic: push-scatter, one barrier, reduce own block (b2_rs.cuh).
 //   * all-to-all with any split sizes: push each block behind a count header, one barrier, copy out (b2_a2a.cuh).
+//   * point-to-point send / recv in batches: per-channel slot inboxes with flags and credits, no barrier (b2_p2p.cuh).
 //   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
 //   * the elementwise passes of training-mode BatchNorm2d on channels-last bf16 activations (b2_bn.cuh).
 //
@@ -35,6 +36,7 @@
 #include "b2_exact.cuh"
 #include "b2_rs.cuh"
 #include "b2_a2a.cuh"
+#include "b2_p2p.cuh"
 #include "b2_bnstats.cuh"
 #include "b2_bn.cuh"
 #include "b2_vmm.h"
@@ -152,7 +154,7 @@ struct b2_comm {
   bool use_vmm = false;        // arena built from VMM objects (else cudaMalloc [+ CUDA IPC])
   bool peer_is_ipc[B2_MAX_WORLD] = {};
   uint8_t* arena_of[B2_MAX_WORLD] = {};  // arena_of[r] = rank r's arena as mapped in this process
-  void* arena = nullptr;       // this rank's arena: [xbar flags | pipeline flags | stage0 | stage1]
+  void* arena = nullptr;       // this rank's arena: [xbar flags | pipeline flags | stage0 | stage1 | LL0 | LL1 | p2p]
   size_t arena_bytes = 0;
   size_t stage_bytes = 0;
   vmm::Mapping own;                  // VMM backend: my physical allocation + its mapping
@@ -160,6 +162,8 @@ struct b2_comm {
   vmm::Mapping mc;                   // VMM backend, multi-process: the multicast object
   LocalMc* local_mc = nullptr;       // VMM backend, in-process world
   uint32_t* counters = nullptr;  // cudaMalloc'ed: opseq, done
+  uint32_t* p2p_counters = nullptr;  // cudaMalloc'ed: chunks sent to [0, W) / received from [8, 8 + W) each rank; [32] done
+  size_t p2p_off = 0;                // the point-to-point region of every arena (b2_p2p.cuh)
   unsigned long long* trace_dev = nullptr;  // cudaMalloc'ed on demand: kMaxCtas * 8 stamps
   uint32_t* status_host = nullptr;
   // tuning (identical on every rank: they come from the same environment / the same b2_comm_set_param calls)
@@ -229,6 +233,9 @@ void layout(b2_comm* c, int world, size_t stage_bytes) {
   c->d.ll_off[1] = c->arena_bytes + ll_bytes;
   c->arena_bytes += 2 * ll_bytes;
   c->d.llflag_off = 32u << 10;  // inside the xbar flag region, past its kMaxCtas slots
+  // point-to-point inboxes, flags and credits: after everything the collectives use, a function of the world size alone
+  c->p2p_off = c->arena_bytes;
+  c->arena_bytes += p2p_region_bytes(world);
 }
 
 // Everything of a rank except the arena itself.
@@ -257,6 +264,8 @@ int init_rank(b2_comm* c, int rank, int world, int device, size_t stage_bytes) {
   B2_CUDA(cudaMemset(c->counters, 0, 256));
   c->d.opseq = c->counters;
   c->d.done = c->counters + 32;  // a different 128 B line
+  B2_CUDA(cudaMalloc(&c->p2p_counters, 256));
+  B2_CUDA(cudaMemset(c->p2p_counters, 0, 256));
   B2_CUDA(cudaHostAlloc(&c->status_host, 64, cudaHostAllocMapped | cudaHostAllocPortable));
   memset(c->status_host, 0, 64);
   void* sdev = nullptr;
@@ -284,6 +293,7 @@ int alloc_arena(b2_comm* c, bool use_vmm, bool multicast, const int* devices, in
   }
   B2_CUDA(cudaMemset(c->arena, 0, kFlagRegionBytes));
   B2_CUDA(cudaMemset(static_cast<uint8_t*>(c->arena) + c->d.ll_off[0], 0xFF, 4 * static_cast<size_t>(c->d.world) * c->d.slice_cap));
+  B2_CUDA(cudaMemset(static_cast<uint8_t*>(c->arena) + c->p2p_off, 0, 2 * p2p_lines_bytes(c->d.world)));  // flags and credits
   B2_CUDA(cudaDeviceSynchronize());
   c->arena_of[c->d.rank] = static_cast<uint8_t*>(c->arena);
   return B2_OK;
@@ -308,11 +318,13 @@ void free_rank_resources(b2_comm* c) {
     cudaFree(c->arena);
   }
   if (c->counters) cudaFree(c->counters);
+  if (c->p2p_counters) cudaFree(c->p2p_counters);
   if (c->trace_dev) cudaFree(c->trace_dev);
   c->trace_dev = nullptr;
   if (c->status_host) cudaFreeHost(c->status_host);
   c->arena = nullptr;
   c->counters = nullptr;
+  c->p2p_counters = nullptr;
   c->status_host = nullptr;
 }
 
@@ -527,14 +539,20 @@ bool wait_count(std::atomic<int>& ctr, int target, std::atomic<int>* abort_flag,
   return true;
 }
 
-// What a kernel records in the status word: B2_ETIMEOUT (a peer wait gave up) or B2_EINVAL (k_alltoall), which says:
+// What a kernel records in the status word: B2_ETIMEOUT (a peer wait gave up) or B2_EINVAL, which says (by status word 1,
+// which k_p2p sets to kStatusP2p before it records B2_EINVAL):
 constexpr const char* kA2aStatusText = "an all-to-all's split sizes disagreed across ranks or exceeded the per-pair limit";
+constexpr const char* kP2pStatusText = "a point-to-point receive's byte count disagreed with its sender's";
+
+const char* einval_text(const b2_comm* c) {
+  return reinterpret_cast<volatile uint32_t*>(c->status_host)[1] == kStatusP2p ? kP2pStatusText : kA2aStatusText;
+}
 
 // A kernel that gave up waiting for a peer leaves the communicator's buffers and counters in an unknown state.  An
 // all-to-all that gave up its exchange leaves them consistent, but the outputs of that call are not written.
 int check_not_poisoned(const b2_comm* c) {
   const uint32_t s = *reinterpret_cast<volatile uint32_t*>(c->status_host);
-  if (s == static_cast<uint32_t>(-B2_EINVAL)) return fail(B2_ESTATE, "communicator poisoned: %s", kA2aStatusText);
+  if (s == static_cast<uint32_t>(-B2_EINVAL)) return fail(B2_ESTATE, "communicator poisoned: %s", einval_text(c));
   if (s != 0) return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
   return B2_OK;
 }
@@ -1012,7 +1030,7 @@ int b2_comm_status(const b2_comm_t* c) {
   const uint32_t s = *reinterpret_cast<volatile uint32_t*>(c->status_host);
   if (s == 0) return B2_OK;
   return fail(-static_cast<int>(s), "rank %d: %s (code %d)", c->d.rank,
-              s == static_cast<uint32_t>(-B2_EINVAL) ? kA2aStatusText : "a kernel gave up waiting for a peer", -static_cast<int>(s));
+              s == static_cast<uint32_t>(-B2_EINVAL) ? einval_text(c) : "a kernel gave up waiting for a peer", -static_cast<int>(s));
 }
 
 uint64_t b2_comm_launch_count(const b2_comm_t* c) { return c ? c->launches : 0; }
@@ -1540,6 +1558,81 @@ int b2_alltoall(b2_comm_t* c, void* const* out, const size_t* recv_bytes, const 
   if (e != cudaSuccess) return fail(B2_ECUDA, "all-to-all kernel launch: %s", cudaGetErrorString(e));
   c->launches++;
   return rc;
+}
+
+size_t b2_p2p_eager_bytes(const b2_comm_t* c) { return c ? kP2pSlots * kP2pPayload : 0; }
+
+int b2_p2p(b2_comm_t* c, const b2_p2p_op_t* ops, int n_ops, void* stream) {
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!ops) return fail(B2_EINVAL, "b2_p2p: null op list");
+  if (n_ops < 1 || n_ops > B2_P2P_MAX_OPS) return fail(B2_EINVAL, "b2_p2p: need 1..%d ops (got %d)", B2_P2P_MAX_OPS, n_ops);
+  const int W = c->d.world, me = c->d.rank;
+  for (int i = 0; i < n_ops; ++i) {
+    if (ops[i].peer < 0 || ops[i].peer >= W || ops[i].peer == me)
+      return fail(B2_EINVAL, "b2_p2p: op %d names peer %d; rank %d of %d can only name another rank", i, ops[i].peer, me, W);
+    if (!ops[i].ptr && ops[i].bytes) return fail(B2_EINVAL, "b2_p2p: op %d has a null pointer and %zu bytes", i, ops[i].bytes);
+  }
+  for (int i = 0; i < n_ops; ++i) {
+    if (ops[i].is_send || !ops[i].bytes) continue;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(ops[i].ptr);
+    for (int j = 0; j < n_ops; ++j) {
+      const uintptr_t b = reinterpret_cast<uintptr_t>(ops[j].ptr);
+      if (j != i && ops[j].bytes && a < b + ops[j].bytes && b < a + ops[i].bytes)
+        return fail(B2_EINVAL, "b2_p2p: op %d (a recv) overlaps op %d", i, j);
+    }
+  }
+  if (const int rc = check_not_poisoned(c)) return rc;
+  // Channels in order of first appearance; an op's chunks follow the chunks of the earlier ops on its channel.
+  P2pArgs a{};
+  int chan_peer[kP2pMaxChans];
+  unsigned long long vecs = 0;
+  for (int i = 0; i < n_ops; ++i) {
+    const int peer = ops[i].peer, send = ops[i].is_send != 0;
+    int k = 0;
+    while (k < a.nchan && !(chan_peer[k] == peer && a.chan[k].send == send)) ++k;
+    if (k == a.nchan) {
+      const int q_me = me < peer ? me : me - 1;  // my block in the peer's arena
+      const int q_peer = peer < me ? peer : peer - 1;  // the peer's block in mine
+      uint8_t* recv_arena = c->arena_of[send ? peer : me] + c->p2p_off;
+      uint8_t* send_arena = c->arena_of[send ? me : peer] + c->p2p_off;
+      const int q_recv = send ? q_me : q_peer;  // the sender's block at the receiver
+      const int q_send = send ? q_peer : q_me;  // the receiver's block at the sender
+      P2pChan& ch = a.chan[a.nchan++];
+      chan_peer[k] = peer;
+      ch.inbox = recv_arena + 2 * p2p_lines_bytes(W) + static_cast<size_t>(q_recv) * kP2pSlots * kP2pSlotBytes;
+      ch.flag = reinterpret_cast<uint32_t*>(recv_arena + static_cast<size_t>(q_recv) * kP2pSlots * kP2pLineBytes);
+      ch.credit = reinterpret_cast<uint32_t*>(send_arena + p2p_lines_bytes(W) + static_cast<size_t>(q_send) * kP2pSlots * kP2pLineBytes);
+      ch.count = c->p2p_counters + (send ? 0 : 8) + peer;
+      ch.send = send;
+      ch.nchunks = 0;
+    }
+    const unsigned long long nch = ops[i].bytes ? (ops[i].bytes + kP2pPayload - 1) / kP2pPayload : 1;
+    P2pOp& op = a.op[i];
+    op.ptr = static_cast<uint8_t*>(ops[i].ptr);
+    op.bytes = ops[i].bytes;
+    op.chan = static_cast<uint32_t>(k);
+    op.chunk0 = a.chan[k].nchunks;
+    op.nchunks = static_cast<uint32_t>(nch);
+    a.chan[k].nchunks += static_cast<uint32_t>(nch);
+    vecs += (ops[i].bytes + 15) / 16;
+  }
+  a.nops = n_ops;
+  // At least one CTA per channel; the heuristic grid (or max_ctas) split evenly beyond that, and never more CTAs than chunks.
+  const int per = grid_for(c, vecs, 1) / a.nchan;
+  int grid = 0;
+  for (int k = 0; k < a.nchan; ++k) {
+    a.chan[k].cta_begin = grid;
+    grid += static_cast<int>(per < 1 ? 1 : (static_cast<uint32_t>(per) < a.chan[k].nchunks ? static_cast<uint32_t>(per) : a.chan[k].nchunks));
+  }
+  a.done = c->p2p_counters + 32;
+  a.status = c->d.status;
+  a.timeout_ns = c->d.timeout_ns;
+  DeviceGuard g(c->device);
+  k_p2p<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "point-to-point kernel launch: %s", cudaGetErrorString(e));
+  c->launches++;
+  return B2_OK;
 }
 
 int b2_batchnorm_stats(b2_comm_t* c, float* mean, float* invstd, float count, size_t channels, float* running_mean,

@@ -96,6 +96,8 @@ SYMBOLS = [
     "b2_reduce_scatter_step",
     "b2_alltoall",
     "b2_alltoall_max_bytes",
+    "b2_p2p",
+    "b2_p2p_eager_bytes",
     "b2_batchnorm_stats",
     "b2_bn_forward_elemt",
     "b2_bn_backward_elemt",
@@ -114,6 +116,15 @@ class B2Segment(ctypes.Structure):
     """b2_segment_t: bucket elements [begin, end) live at device pointer src."""
 
     _fields_ = [("src", ctypes.c_void_p), ("begin", ctypes.c_uint64), ("end", ctypes.c_uint64)]
+
+
+B2_P2P_MAX_OPS = 64
+
+
+class B2P2pOp(ctypes.Structure):
+    """b2_p2p_op_t: one send (is_send != 0) or receive of `bytes` bytes at device pointer ptr, to or from rank peer."""
+
+    _fields_ = [("peer", ctypes.c_int), ("is_send", ctypes.c_int), ("ptr", ctypes.c_void_p), ("bytes", ctypes.c_size_t)]
 
 
 B2_OPT_SGD = 1
@@ -225,6 +236,10 @@ def lib() -> ctypes.CDLL:
     L.b2_alltoall.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(vp), ctypes.POINTER(sz), vp]
     L.b2_alltoall_max_bytes.restype = sz
     L.b2_alltoall_max_bytes.argtypes = [vp]
+    L.b2_p2p.restype = i
+    L.b2_p2p.argtypes = [vp, ctypes.POINTER(B2P2pOp), i, vp]
+    L.b2_p2p_eager_bytes.restype = sz
+    L.b2_p2p_eager_bytes.argtypes = [vp]
     L.b2_batchnorm_stats.restype = i
     L.b2_batchnorm_stats.argtypes = [vp, vp, vp, f, sz, vp, vp, ctypes.c_double, ctypes.c_double, vp, vp]
     L.b2_bn_forward_elemt.restype = i

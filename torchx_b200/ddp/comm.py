@@ -8,6 +8,7 @@ torch is used for tensors and streams only.
 from __future__ import annotations
 
 import ctypes
+import operator
 import os
 from typing import List, Optional, Sequence
 
@@ -56,6 +57,16 @@ def dtype_op_for(dtype: torch.dtype, op: str, fn: str = "allreduce_op_"):
     if op == "avg" and not dtype.is_floating_point:
         raise TypeError(f"{fn}: avg needs a floating-point tensor, got {dtype}")
     return EXACT_DTYPES[dtype], REDUCE_OPS[op]
+
+
+def as_rank(x) -> Optional[int]:
+    """``x`` as a rank number if it is an integer as torch takes one (a Python or numpy integer, not a bool), else None."""
+    if isinstance(x, bool):
+        return None
+    try:
+        return operator.index(x)
+    except TypeError:
+        return None
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream], device: int) -> int:
@@ -179,6 +190,12 @@ class Communicator:
         """The most bytes one rank may send another in one ``alltoall_`` (b2_alltoall_max_bytes)."""
         return int(N.lib().b2_alltoall_max_bytes(self._h))
 
+    @property
+    def p2p_eager_bytes(self) -> int:
+        """The largest message a ``p2p_`` send completes without its receive having been launched, once the earlier
+        messages to that rank have been received (b2_p2p_eager_bytes)."""
+        return int(N.lib().b2_p2p_eager_bytes(self._h))
+
     # ---- collectives ---------------------------------------------------------------------------
     def allreduce_(self, t: torch.Tensor, scale: Optional[float] = None, wire: str = "bf16", algo: str = "auto",
                    stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
@@ -298,6 +315,28 @@ class Communicator:
         N.check(N.lib().b2_alltoall(self._h, ptrs(outs), sizes(outs), ptrs(ins), sizes(ins),
                                     ctypes.c_void_p(_stream_ptr(stream, self.device))))
         return outs
+
+    def p2p_(self, ops: Sequence, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """One batch of point-to-point operations in one launch (include/b200ddp.h: b2_p2p).  ``ops`` is a list of 1..64
+        ``("send" | "recv", tensor, peer)``: a send gives the tensor's bytes to rank ``peer``, a recv fills the tensor with the
+        next message rank ``peer`` sends this rank, which must have as many bytes.  Messages between two ranks match in issue
+        order; the ops of one batch make progress whatever their order.  Tensors are contiguous, on this communicator's
+        device, of any dtype; a recv tensor may not overlap any other tensor of the batch."""
+        if not 1 <= len(ops) <= N.B2_P2P_MAX_OPS:
+            raise ValueError(f"p2p_: needs 1..{N.B2_P2P_MAX_OPS} ops, got {len(ops)}")
+        peers = []
+        for k, (kind, _, peer) in enumerate(ops):
+            if kind not in ("send", "recv"):
+                raise ValueError(f"p2p_: op {k} is {kind!r}, not 'send' or 'recv'")
+            p = as_rank(peer)
+            if p is None or not 0 <= p < self.world or p == self.rank:
+                raise ValueError(f"p2p_: op {k} names peer {peer!r}; rank {self.rank} of {self.world} can only name another rank")
+            peers.append(p)
+        arr = (N.B2P2pOp * len(ops))()
+        for k, ((kind, t, _), peer) in enumerate(zip(ops, peers)):
+            self._check_tensor(t)
+            arr[k] = N.B2P2pOp(peer, int(kind == "send"), t.data_ptr(), t.numel() * t.element_size())
+        N.check(N.lib().b2_p2p(self._h, arr, len(ops), ctypes.c_void_p(_stream_ptr(stream, self.device))))
 
     def batchnorm_stats_(self, mean: torch.Tensor, invstd: torch.Tensor, count: float, running_mean: Optional[torch.Tensor] = None,
                          running_var: Optional[torch.Tensor] = None, *, momentum: float, eps: float,

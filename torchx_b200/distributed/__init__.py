@@ -8,7 +8,8 @@ environment contract and barrier-ordered critical sections.  Two backends behind
     otherwise) - this is what config #1 (CPU/gloo) and unmodified TorchX scripts use;
   * ``init_pg("b200")`` - the peer-buffer communicator from ``libb200ddp.so``: no TCP store, no NCCL.  ``barrier`` /
     ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor``, ``all_gather``, ``reduce_scatter_tensor``,
-    ``reduce_scatter``, ``broadcast``, ``all_to_all_single`` and ``all_to_all`` then run on that fabric.
+    ``reduce_scatter``, ``broadcast``, ``all_to_all_single``, ``all_to_all``, the point-to-point ``send``, ``recv``,
+    ``isend``, ``irecv``, ``P2POp`` / ``batch_isend_irecv``, and ``gather`` / ``scatter`` then run on that fabric.
 """
 from __future__ import annotations
 
@@ -259,6 +260,171 @@ def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[t
     _check_native_call(group, async_op)
     _COMM.alltoall_(output_tensor_list, input_tensor_list)
     return None
+
+
+def send(tensor: torch.Tensor, dst: int, group: Any = None, tag: int = 0) -> None:
+    """``torch.distributed.send``: rank ``dst`` receives ``tensor``'s bytes.  Under ``init_pg("b200")`` it is enqueued on the
+    current stream (as NCCL's is) and messages to one rank match that rank's receives in issue order; ``tag`` is accepted
+    and ignored, as torch's NCCL backend does."""
+    if not _on_fabric():
+        return dist.send(tensor, dst, group=group, tag=tag)
+    _check_native_call(group, False)
+    _COMM.p2p_([("send", tensor, dst)])
+    return None
+
+
+def recv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0) -> int:
+    """``torch.distributed.recv``: ``tensor`` <- the next message rank ``src`` sends this rank (it must have as many bytes);
+    returns ``src``.  Receiving from any rank (``src=None``) is not available on the fabric."""
+    if not _on_fabric():
+        return dist.recv(tensor, src, group=group, tag=tag)
+    _check_native_call(group, False)
+    if src is None:
+        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
+    _COMM.p2p_([("recv", tensor, src)])
+    return src
+
+
+class _P2PWork:
+    """The handle of a point-to-point op on the fabric.  The op is enqueued on the stream that was current at the call, so
+    later work on that stream is already ordered after it: ``wait()`` returns True at once.  ``is_completed()`` asks
+    whether the GPU has finished it."""
+
+    def __init__(self, event: torch.cuda.Event) -> None:
+        self._event = event
+
+    def wait(self, timeout: Any = None) -> bool:
+        return True
+
+    def is_completed(self) -> bool:
+        return self._event.query()
+
+
+def _p2p_batch(ops: List[Any]) -> _P2PWork:
+    _COMM.p2p_(ops)
+    event = torch.cuda.Event()
+    event.record(torch.cuda.current_stream(_COMM.device))
+    return _P2PWork(event)
+
+
+def isend(tensor: torch.Tensor, dst: int, group: Any = None, tag: int = 0) -> Any:
+    """``torch.distributed.isend``: ``send`` returning a work handle."""
+    if not _on_fabric():
+        return dist.isend(tensor, dst, group=group, tag=tag)
+    _check_native_call(group, False)
+    return _p2p_batch([("send", tensor, dst)])
+
+
+def irecv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0) -> Any:
+    """``torch.distributed.irecv``: ``recv`` returning a work handle."""
+    if not _on_fabric():
+        return dist.irecv(tensor, src, group=group, tag=tag)
+    _check_native_call(group, False)
+    if src is None:
+        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
+    return _p2p_batch([("recv", tensor, src)])
+
+
+class P2POp:
+    """``torch.distributed.P2POp``: one entry of ``batch_isend_irecv``.  ``op`` is ``isend`` or ``irecv`` (this module's or
+    torch.distributed's).  Under ``init_pg("b200")`` it is a plain record, so it needs no process group; with one it is
+    ``torch.distributed.P2POp`` itself, built with torch's ``isend`` / ``irecv`` in place of this module's, so a script
+    written with ``P2POp(isend, ...)`` runs under either backend."""
+
+    def __new__(cls, op: Any, tensor: torch.Tensor, peer: Optional[int] = None, group: Any = None, tag: int = 0) -> Any:
+        if not _on_fabric():
+            op = dist.isend if op is isend else (dist.irecv if op is irecv else op)
+            return dist.P2POp(op, tensor, peer, group, tag)
+        if op not in (isend, irecv, dist.isend, dist.irecv):
+            raise ValueError("Invalid ``op``. Expected ``op`` to be of type ``torch.distributed.isend`` or ``torch.distributed.irecv``.")
+        self = super().__new__(cls)
+        self.op, self.tensor, self.peer, self.group, self.tag = op, tensor, peer, group, tag
+        return self
+
+
+def batch_isend_irecv(p2p_op_list: List[Any]) -> List[Any]:
+    """``torch.distributed.batch_isend_irecv``: every op of the list in ONE launch under ``init_pg("b200")``, one handle per
+    op.  A list longer than the fabric's 64 ops is refused rather than split: the ops of one launch cannot wait on each
+    other, and split launches could."""
+    if not _on_fabric():
+        return dist.batch_isend_irecv(p2p_op_list)
+    from torchx_b200.ddp._native import B2_P2P_MAX_OPS
+
+    if not p2p_op_list:
+        raise ValueError("batch_isend_irecv: p2p_op_list is empty")
+    if len(p2p_op_list) > B2_P2P_MAX_OPS:
+        raise ValueError(f"batch_isend_irecv: {len(p2p_op_list)} ops, the b200 communicator takes at most {B2_P2P_MAX_OPS} "
+                         "in one batch")
+    ops = []
+    for p in p2p_op_list:
+        _check_native_call(p.group, False)
+        if p.peer is None:
+            raise NotImplementedError("the b200 communicator cannot receive from any source: pass peer")
+        ops.append(("send" if p.op in (isend, dist.isend) else "recv", p.tensor, p.peer))
+    work = _p2p_batch(ops)
+    return [work] * len(ops)
+
+
+def _check_rank(name: str, r: Any) -> int:
+    from torchx_b200.ddp.comm import as_rank
+
+    k = as_rank(r)
+    if k is None or not 0 <= k < _COMM.world:
+        raise ValueError(f"{name} {r!r} is not a rank of a world of {_COMM.world}")
+    return k
+
+
+def gather(tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]] = None, dst: int = 0, group: Any = None,
+           async_op: bool = False) -> Any:
+    """``torch.distributed.gather``: on rank ``dst``, ``gather_list[r]`` <- rank r's ``tensor``.  Under ``init_pg("b200")``
+    rank ``dst`` runs one batch of W - 1 receives and copies its own tensor; every other rank runs one send."""
+    if not _on_fabric():
+        return dist.gather(tensor, gather_list, dst=dst, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    dst = _check_rank("gather: dst", dst)
+    if _COMM.rank != dst:
+        if gather_list:
+            raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
+        _COMM.p2p_([("send", tensor, dst)])
+        return None
+    if not gather_list:
+        raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
+    _check_list("gather: gather_list", gather_list, tensor)
+    if _COMM.world > 1:
+        _COMM.p2p_([("recv", t, r) for r, t in enumerate(gather_list) if r != dst])
+    gather_list[dst].copy_(tensor)
+    return None
+
+
+def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = None, src: int = 0, group: Any = None,
+            async_op: bool = False) -> Any:
+    """``torch.distributed.scatter``: every rank r's ``tensor`` <- ``scatter_list[r]`` of rank ``src``.  Under
+    ``init_pg("b200")`` rank ``src`` runs one batch of W - 1 sends and copies its own block; every other rank runs one
+    receive."""
+    if not _on_fabric():
+        return dist.scatter(tensor, scatter_list, src=src, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    src = _check_rank("scatter: src", src)
+    if _COMM.rank != src:
+        if scatter_list:
+            raise ValueError("Argument ``scatter_list`` must NOT be specified on non-source ranks.")
+        _COMM.p2p_([("recv", tensor, src)])
+        return None
+    if not scatter_list:
+        raise ValueError("Argument ``scatter_list`` must be specified on source rank.")
+    _check_list("scatter: scatter_list", scatter_list, tensor)
+    if _COMM.world > 1:
+        _COMM.p2p_([("send", t, r) for r, t in enumerate(scatter_list) if r != src])
+    tensor.copy_(scatter_list[src])
+    return None
+
+
+def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor) -> None:
+    if len(tensors) != _COMM.world:
+        raise ValueError(f"{what} has {len(tensors)} tensors, world size is {_COMM.world}")
+    for t in tensors:
+        if t.dtype != like.dtype or t.numel() != like.numel():
+            raise ValueError(f"{what}: every tensor must be {like.dtype} with {like.numel()} elements")
 
 
 @contextmanager
