@@ -379,15 +379,26 @@ PipePlan plan_pipe(const b2_comm* c, unsigned long long Ls, size_t wire_bytes) {
   return p;
 }
 
-// One collective of `kind` (B2_ALGO_ONESHOT / TWOSHOT / TWOSHOT_PIPE / TWOSHOT_LL / NVLS) at the communicator's world
-// size: instantiates the collective kernels of MODE for W = 2 .. B2_MAX_WORLD.
-template <int MODE, int W = 2>
+// The world sizes of the multi-rank kernels: calls f(std::integral_constant<int, W>{}) and returns true for
+// W = world in 2 .. B2_MAX_WORLD, or returns false.  Every runtime world size becomes a compile-time one here.
+template <int W = 2, class F>
+bool with_world(int world, F&& f) {
+  if constexpr (W > B2_MAX_WORLD) {
+    return false;
+  } else {
+    if (world != W) return with_world<W + 1>(world, f);
+    f(std::integral_constant<int, W>{});
+    return true;
+  }
+}
+
+// One collective of `kind` (B2_ALGO_ONESHOT / TWOSHOT / TWOSHOT_PIPE / TWOSHOT_LL / NVLS) at the communicator's world size.
+template <int MODE>
 cudaError_t launch_collective(const CommDev& d, const Src& src, int kind, int grid, const PipePlan& p, void* buf,
                               unsigned long long n, float scale, cudaStream_t s) {
-  if constexpr (W > B2_MAX_WORLD) {
-    return cudaErrorInvalidValue;
-  } else {
-    if (d.world != W) return launch_collective<MODE, W + 1>(d, src, kind, grid, p, buf, n, scale, s);
+  cudaError_t e = cudaErrorInvalidValue;
+  with_world(d.world, [&](auto w) {
+    constexpr int W = decltype(w)::value;
     switch (kind) {
       case B2_ALGO_ONESHOT:
         k_oneshot<MODE, W><<<grid, kThreads, 0, s>>>(d, src, buf, n, scale);
@@ -404,35 +415,31 @@ cudaError_t launch_collective(const CommDev& d, const Src& src, int kind, int gr
       default:  // B2_ALGO_NVLS
         k_pipe<MODE, W, pl::kNvls><<<p.grid, kThreads, 0, s>>>(d, src, buf, n, scale, p.K, p.cell);
     }
-    return cudaGetLastError();
-  }
+    e = cudaGetLastError();
+  });
+  return e;
 }
 
-// The float reduce-scatter at the communicator's world size: instantiates k_reduce_scatter<MODE, W> for the five gradient
-// modes and W = 2 .. B2_MAX_WORLD.
-template <int MODE, int W = 2>
+// The float reduce-scatter at the communicator's world size.
+template <int MODE>
 cudaError_t launch_reduce_scatter(const CommDev& d, const Src& src, int grid, void* out, const void* in, unsigned long long n,
                                   unsigned long long block, float scale, cudaStream_t s) {
-  if constexpr (W > B2_MAX_WORLD) {
-    return cudaErrorInvalidValue;
-  } else {
-    if (d.world != W) return launch_reduce_scatter<MODE, W + 1>(d, src, grid, out, in, n, block, scale, s);
-    k_reduce_scatter<MODE, W><<<grid, kThreads, 0, s>>>(d, src, out, in, n, block, scale);
-    return cudaGetLastError();
-  }
+  cudaError_t e = cudaErrorInvalidValue;
+  with_world(d.world, [&](auto w) {
+    k_reduce_scatter<MODE, decltype(w)::value><<<grid, kThreads, 0, s>>>(d, src, out, in, n, block, scale);
+    e = cudaGetLastError();
+  });
+  return e;
 }
 
-// The optimizer-fused reduce-scatter at the communicator's world size (fp32-bucket modes only).
-template <int MODE, int W = 2>
-cudaError_t launch_reduce_scatter_step(const CommDev& d, const Src& src, const OptDev& o, int grid, unsigned long long n,
-                                       unsigned long long block, float scale, cudaStream_t s) {
-  if constexpr (W > B2_MAX_WORLD) {
-    return cudaErrorInvalidValue;
-  } else {
-    if (d.world != W) return launch_reduce_scatter_step<MODE, W + 1>(d, src, o, grid, n, block, scale, s);
-    k_reduce_scatter_step<MODE, W><<<grid, kThreads, 0, s>>>(d, src, o, n, block, scale);
-    return cudaGetLastError();
-  }
+// The local pass's grid over n elements: enough CTAs for 4 vecs per thread, at most 4 resident CTAs per SM (~64 KiB of
+// loads in flight per SM).
+int local_grid(unsigned long long n, unsigned long long sms) {
+  const unsigned long long V = (n + 7) / 8;
+  unsigned long long g = (V + kThreads * 4ull - 1) / (kThreads * 4ull);
+  if (g < 1) g = 1;
+  if (g > sms * 4) g = sms * 4;
+  return static_cast<int>(g);
 }
 
 template <int MODE>
@@ -460,11 +467,7 @@ cudaError_t launch_local(const Src& src, void* buf, unsigned long long n, float 
     k_local_pass_tma<MODE><<<static_cast<int>(g), tma::kTmaThreads, kSmem, s>>>(buf, n, scale);
     return cudaGetLastError();
   }
-  const unsigned long long V = (n + 7) / 8;
-  unsigned long long g = (V + kThreads * 4ull - 1) / (kThreads * 4ull);
-  if (g < 1) g = 1;
-  if (g > sms * 4) g = sms * 4;  // 4 resident CTAs per SM keep ~64 KiB of loads in flight per SM
-  k_local_pass<MODE><<<static_cast<int>(g), kThreads, 0, s>>>(src, buf, n, scale);
+  k_local_pass<MODE><<<local_grid(n, sms), kThreads, 0, s>>>(src, buf, n, scale);
   return cudaGetLastError();
 }
 
@@ -511,6 +514,26 @@ size_t wire_vec_bytes(int mode) {
 
 const Src kNoSrc = {};  // nseg == 0: the collective reads the bucket itself
 
+// Calls launch(off, n) for the consecutive chunks [off, off + n) of [0, total), each of at most cap units, and counts each
+// launch on c.  launch returns its launch error; the first failure ends the loop and is returned.
+template <class F>
+cudaError_t for_chunks(b2_comm* c, size_t total, size_t cap, F&& launch) {
+  for (size_t off = 0; off < total;) {
+    const size_t n = total - off < cap ? total - off : cap;
+    const cudaError_t e = launch(off, n);
+    if (e != cudaSuccess) return e;
+    c->launches++;
+    off += n;
+  }
+  return cudaSuccess;
+}
+
+// [p, p + n) and [q, q + m) share a byte (an empty range shares none).
+bool overlaps(const void* p, size_t n, const void* q, size_t m) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+  return n && m && a < b + m && b < a + n;
+}
+
 int local_pass_impl(const Src& src, void* buf, size_t n_elems, int mode, float scale, int device, void* stream) {
   if (n_elems == 0) return B2_OK;
   if (!buf) return fail(B2_EINVAL, "b2_local_pass: null buffer");
@@ -537,6 +560,17 @@ bool wait_count(std::atomic<int>& ctr, int target, std::atomic<int>* abort_flag,
     usleep(200);
   }
   return true;
+}
+
+// Waits until `flag` (&ShmSlot::hello or &ShmSlot::ready) is set in every rank's slot of the control block.
+int wait_slots(const b2_comm* c, std::atomic<uint32_t> ShmSlot::*flag, double deadline) {
+  for (int r = 0; r < c->d.world; ++r) {
+    while ((c->shm->slot[r].*flag).load(std::memory_order_acquire) != 1) {
+      if (now_s() > deadline) return fail(B2_ETIMEOUT, "rendezvous timed out waiting for rank %d on %s", r, c->shm_path.c_str());
+      usleep(200);
+    }
+  }
+  return B2_OK;
 }
 
 // What a kernel records in the status word: B2_ETIMEOUT (a peer wait gave up) or B2_EINVAL, which says (by status word 1,
@@ -818,14 +852,8 @@ int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char*
     }
     me.hello.store(1, std::memory_order_release);
     bool use_vmm = true, use_mc = true;
+    rc = wait_slots(c, &ShmSlot::hello, deadline);
     for (int r = 0; r < world && rc == B2_OK; ++r) {
-      while (sb->slot[r].hello.load(std::memory_order_acquire) != 1) {
-        if (now_s() > deadline) {
-          rc = fail(B2_ETIMEOUT, "rendezvous timed out waiting for rank %d on %s", r, c->shm_path.c_str());
-          break;
-        }
-        usleep(200);
-      }
       use_vmm = use_vmm && sb->slot[r].cap_vmm != 0;
       use_mc = use_mc && sb->slot[r].cap_mc != 0;
     }
@@ -845,15 +873,7 @@ int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char*
       me.arena_bytes = c->arena_bytes;
       if (rc == B2_OK) me.ready.store(1, std::memory_order_release);
     }
-    for (int r = 0; r < world && rc == B2_OK; ++r) {
-      while (sb->slot[r].ready.load(std::memory_order_acquire) != 1) {
-        if (now_s() > deadline) {
-          rc = fail(B2_ETIMEOUT, "rendezvous timed out waiting for rank %d on %s", r, c->shm_path.c_str());
-          break;
-        }
-        usleep(200);
-      }
-    }
+    if (rc == B2_OK) rc = wait_slots(c, &ShmSlot::ready, deadline);
     // ---- 3. map every peer's arena -------------------------------------------------------------------------
     int stash_mc_fd = -1;
     for (int r = 0; r < world && rc == B2_OK; ++r) {
@@ -1169,19 +1189,16 @@ int b2_reduce_scatter_gather(b2_comm_t* c, void* out, size_t block, const b2_seg
   const size_t eb = elem_bytes(mode);
   const size_t cap = c->d.slice_cap / wire_vec_bytes(mode) * 8;  // elements of a block one recv region holds (whole vecs)
   uint8_t* po = static_cast<uint8_t*>(out);
-  size_t off = 0;
-  while (off < block) {
-    const size_t n = block - off < cap ? block - off : cap;
+  const cudaError_t e = for_chunks(c, block, cap, [&](size_t off, size_t n) {
     const int grid = grid_for(c, (n + 7) / 8, vecs_per_trip(W));
     src.off = off;  // every block's launch-local element 0 is bucket element j * block + off
-    cudaError_t e = cudaErrorInvalidValue;  // never guess a mode
+    cudaError_t le = cudaErrorInvalidValue;  // never guess a mode
     with_mode(mode, [&](auto m) {
-      e = launch_reduce_scatter<decltype(m)::value>(c->d, src, grid, po + off * eb, nullptr, n, block, scale, s);
+      le = launch_reduce_scatter<decltype(m)::value>(c->d, src, grid, po + off * eb, nullptr, n, block, scale, s);
     });
-    if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
-    c->launches++;
-    off += n;
-  }
+    return le;
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -1261,33 +1278,29 @@ int b2_reduce_scatter_step(b2_comm_t* c, size_t block, const b2_segment_t* segme
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  auto step = [&](auto m) -> cudaError_t {
-    constexpr int MODE = decltype(m)::value;
-    if (W == 1) {  // the local pass's grid and rounding
-      const unsigned long long V = (block + 7) / 8;
-      unsigned long long grid = (V + kThreads * 4ull - 1) / (kThreads * 4ull);
-      const unsigned long long cap = 4ull * static_cast<unsigned long long>(sm_count(c->device));
-      grid = grid < 1 ? 1 : (grid > cap ? cap : grid);
-      k_local_step<MODE><<<static_cast<int>(grid), kThreads, 0, s>>>(src, o, block, scale);
-      c->launches++;
-      return cudaGetLastError();
-    }
-    const size_t cap = c->d.slice_cap / dev::Wire<MODE>::kBytes * 8;  // elements of a block one recv region holds
-    for (size_t off = 0; off < block;) {
-      const size_t n = block - off < cap ? block - off : cap;
-      src.off = off;  // the same block offset for the gradient table and the parameter / state slices
-      o.off = off;
-      const cudaError_t e = launch_reduce_scatter_step<MODE>(c->d, src, o, grid_for(c, (n + 7) / 8, 1), n, block, scale, s);
-      if (e != cudaSuccess) return e;
-      c->launches++;
-      off += n;
-    }
-    return cudaSuccess;
-  };
   cudaError_t e = cudaErrorInvalidValue;
-  if (mode == B2_F32_WIRE_BF16) e = step(std::integral_constant<int, B2_F32_WIRE_BF16>{});
-  else if (mode == B2_F32) e = step(std::integral_constant<int, B2_F32>{});
-  else e = step(std::integral_constant<int, B2_F32_WIRE_F16>{});
+  with_mode(mode, [&](auto m) {
+    constexpr int MODE = decltype(m)::value;
+    if constexpr (!k16BitBucket<MODE>) {
+      if (W == 1) {  // the local pass's grid and rounding
+        k_local_step<MODE><<<local_grid(block, sm_count(c->device)), kThreads, 0, s>>>(src, o, block, scale);
+        c->launches++;
+        e = cudaGetLastError();
+        return;
+      }
+      const size_t cap = c->d.slice_cap / dev::Wire<MODE>::kBytes * 8;  // elements of a block one recv region holds
+      e = for_chunks(c, block, cap, [&](size_t off, size_t n) {
+        src.off = off;  // the same block offset for the gradient table and the parameter / state slices
+        o.off = off;
+        cudaError_t le = cudaErrorInvalidValue;
+        with_world(W, [&](auto w) {
+          k_reduce_scatter_step<MODE, decltype(w)::value><<<grid_for(c, (n + 7) / 8, 1), kThreads, 0, s>>>(c->d, src, o, n, block, scale);
+          le = cudaGetLastError();
+        });
+        return le;
+      });
+    }
+  });
   if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter step kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
@@ -1301,18 +1314,11 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
   DeviceGuard g(c->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t cap = c->stage_bytes & ~static_cast<size_t>(15);
-  uint8_t* p = static_cast<uint8_t*>(buf);
-  size_t left = bytes;
-  while (left > 0) {
-    const size_t n = left < cap ? left : cap;
-    const int grid = grid_for(c, (n + 15) / 16, 1);
-    k_broadcast<<<grid, kThreads, 0, s>>>(c->d, p, n, root);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(B2_ECUDA, "broadcast kernel launch: %s", cudaGetErrorString(e));
-    c->launches++;
-    p += n;
-    left -= n;
-  }
+  const cudaError_t e = for_chunks(c, bytes, cap, [&](size_t off, size_t n) {
+    k_broadcast<<<grid_for(c, (n + 15) / 16, 1), kThreads, 0, s>>>(c->d, static_cast<uint8_t*>(buf) + off, n, root);
+    return cudaGetLastError();
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "broadcast kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -1320,51 +1326,62 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
 
 namespace {
 
-const char* dtype_name(int dtype) {
+// The B2_DT_* dtypes of include/b200ddp.h: calls f(std::integral_constant<int, DT>{}) and returns true, or returns false
+// for an unknown dtype.  The only switch over them; what they are is exact::DtypeTraits<DT>.
+template <class F>
+bool with_dtype(int dtype, F&& f) {
   switch (dtype) {
-    case B2_DT_INT32: return "int32";
-    case B2_DT_INT64: return "int64";
-    case B2_DT_FLOAT32: return "float32";
-    case B2_DT_BFLOAT16: return "bfloat16";
-    case B2_DT_FLOAT16: return "float16";
-    default: return nullptr;
+    case B2_DT_INT32: f(std::integral_constant<int, B2_DT_INT32>{}); return true;
+    case B2_DT_INT64: f(std::integral_constant<int, B2_DT_INT64>{}); return true;
+    case B2_DT_FLOAT32: f(std::integral_constant<int, B2_DT_FLOAT32>{}); return true;
+    case B2_DT_BFLOAT16: f(std::integral_constant<int, B2_DT_BFLOAT16>{}); return true;
+    case B2_DT_FLOAT16: f(std::integral_constant<int, B2_DT_FLOAT16>{}); return true;
+    default: return false;
   }
 }
 
-template <int DT, class F>
-bool with_exact_op_of(int op, F&& f) {
-  using Dt = std::integral_constant<int, DT>;
-  switch (op) {
-    case B2_OP_SUM:
-      if constexpr (exact::DtypeTraits<DT>::kInt) {
-        f(Dt{}, std::integral_constant<int, B2_OP_SUM>{});
-        return true;
-      } else {
-        return false;  // float SUM runs on the allreduce kernels
-      }
-    case B2_OP_MIN:
-      f(Dt{}, std::integral_constant<int, B2_OP_MIN>{});
-      return true;
-    case B2_OP_MAX:
-      f(Dt{}, std::integral_constant<int, B2_OP_MAX>{});
-      return true;
-    default:
-      return false;
-  }
+const char* dtype_name(int dtype) {
+  const char* s = nullptr;
+  with_dtype(dtype, [&](auto d) { s = exact::DtypeTraits<decltype(d)::value>::kName; });
+  return s;
+}
+
+size_t dtype_bytes(int dtype) {
+  size_t b = 0;
+  with_dtype(dtype, [&](auto d) { b = exact::DtypeTraits<decltype(d)::value>::kBytes; });
+  return b;
+}
+
+bool dtype_is_int(int dtype) {
+  bool i = false;
+  with_dtype(dtype, [&](auto d) { i = exact::DtypeTraits<decltype(d)::value>::kInt; });
+  return i;
 }
 
 // The (dtype, op) pairs of the exact kernels: calls f(std::integral_constant<int, DT>{}, std::integral_constant<int, OP>{})
-// and returns true, or returns false for float SUM / AVG and anything unknown.  The only switch over them.
+// and returns true, or returns false for float SUM / AVG and anything unknown.
 template <class F>
 bool with_exact_op(int dtype, int op, F&& f) {
-  switch (dtype) {
-    case B2_DT_INT32: return with_exact_op_of<B2_DT_INT32>(op, f);
-    case B2_DT_INT64: return with_exact_op_of<B2_DT_INT64>(op, f);
-    case B2_DT_FLOAT32: return with_exact_op_of<B2_DT_FLOAT32>(op, f);
-    case B2_DT_BFLOAT16: return with_exact_op_of<B2_DT_BFLOAT16>(op, f);
-    case B2_DT_FLOAT16: return with_exact_op_of<B2_DT_FLOAT16>(op, f);
-    default: return false;
-  }
+  bool ok = false;
+  with_dtype(dtype, [&](auto d) {
+    switch (op) {
+      case B2_OP_SUM:
+        if constexpr (exact::DtypeTraits<decltype(d)::value>::kInt) {  // float SUM runs on the allreduce kernels
+          f(d, std::integral_constant<int, B2_OP_SUM>{});
+          ok = true;
+        }
+        break;
+      case B2_OP_MIN:
+        f(d, std::integral_constant<int, B2_OP_MIN>{});
+        ok = true;
+        break;
+      case B2_OP_MAX:
+        f(d, std::integral_constant<int, B2_OP_MAX>{});
+        ok = true;
+        break;
+    }
+  });
+  return ok;
 }
 
 cudaError_t launch_reduce_exact(int dtype, int op, const CommDev& d, int grid, void* buf, unsigned long long n, cudaStream_t s) {
@@ -1375,10 +1392,6 @@ cudaError_t launch_reduce_exact(int dtype, int op, const CommDev& d, int grid, v
   });
   return e;
 }
-
-size_t dtype_bytes(int dtype) { return dtype == B2_DT_INT64 ? 8 : (dtype == B2_DT_BFLOAT16 || dtype == B2_DT_FLOAT16 ? 2 : 4); }
-
-bool dtype_is_int(int dtype) { return dtype == B2_DT_INT32 || dtype == B2_DT_INT64; }
 
 // The B2_* mode of a float SUM / AVG: the gradient mode whose bucket has this dtype and is its own wire format.
 int sum_mode_for(int dtype) { return dtype == B2_DT_FLOAT32 ? B2_F32 : (dtype == B2_DT_BFLOAT16 ? B2_BF16 : B2_F16); }
@@ -1413,17 +1426,10 @@ int b2_allreduce_op(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, 
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t eb = dtype_bytes(dtype);
   const size_t cap = c->d.slice_cap / eb;  // elements one recv region holds (slice_cap is a multiple of 256 bytes)
-  uint8_t* p = static_cast<uint8_t*>(buf);
-  size_t left = n_elems;
-  while (left > 0) {
-    const size_t n = left < cap ? left : cap;
-    const int grid = grid_for(c, (n * eb + 15) / 16, 1);
-    const cudaError_t e = launch_reduce_exact(dtype, op, c->d, grid, p, n, s);
-    if (e != cudaSuccess) return fail(B2_ECUDA, "exact allreduce kernel launch: %s", cudaGetErrorString(e));
-    c->launches++;
-    p += n * eb;
-    left -= n;
-  }
+  const cudaError_t e = for_chunks(c, n_elems, cap, [&](size_t off, size_t n) {
+    return launch_reduce_exact(dtype, op, c->d, grid_for(c, (n * eb + 15) / 16, 1), static_cast<uint8_t*>(buf) + off * eb, n, s);
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "exact allreduce kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -1432,28 +1438,22 @@ int b2_allgather(b2_comm_t* c, void* out, const void* in, size_t bytes, void* st
   if (!c) return fail(B2_EINVAL, "null communicator");
   if (!out || !in) return fail(B2_EINVAL, "b2_allgather: null buffer");
   const int W = c->d.world;
-  const uintptr_t o = reinterpret_cast<uintptr_t>(out), i = reinterpret_cast<uintptr_t>(in);
-  const uintptr_t own = o + static_cast<uintptr_t>(c->d.rank) * bytes;
-  if (i != own && i < o + static_cast<uintptr_t>(W) * bytes && o < i + bytes)
+  const bool in_place = in == static_cast<const uint8_t*>(out) + static_cast<size_t>(c->d.rank) * bytes;
+  if (!in_place && overlaps(in, bytes, out, static_cast<size_t>(W) * bytes))
     return fail(B2_EINVAL, "b2_allgather: `in` overlaps `out` other than as this rank's block");
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (W == 1) {
-    if (i != own) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
+    if (!in_place) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
     return B2_OK;
   }
-  const size_t cap = c->d.slice_cap;
-  size_t off = 0;
-  while (off < bytes) {
-    const size_t n = bytes - off < cap ? bytes - off : cap;
-    const int grid = grid_for(c, (n + 15) / 16, 1);
-    k_allgather<<<grid, kThreads, 0, s>>>(c->d, static_cast<uint8_t*>(out) + off, static_cast<const uint8_t*>(in) + off, n, bytes);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return fail(B2_ECUDA, "all-gather kernel launch: %s", cudaGetErrorString(e));
-    c->launches++;
-    off += n;
-  }
+  const cudaError_t e = for_chunks(c, bytes, c->d.slice_cap, [&](size_t off, size_t n) {
+    k_allgather<<<grid_for(c, (n + 15) / 16, 1), kThreads, 0, s>>>(c->d, static_cast<uint8_t*>(out) + off,
+                                                                   static_cast<const uint8_t*>(in) + off, n, bytes);
+    return cudaGetLastError();
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "all-gather kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -1465,15 +1465,14 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
   const int W = c->d.world;
   const size_t eb = dtype_bytes(dtype);
   const size_t bytes = n_elems * eb;  // one block
-  const uintptr_t o = reinterpret_cast<uintptr_t>(out), i = reinterpret_cast<uintptr_t>(in);
-  const uintptr_t own = i + static_cast<uintptr_t>(c->d.rank) * bytes;
-  if (o != own && o < i + static_cast<uintptr_t>(W) * bytes && i < o + bytes)
+  const bool in_place = out == static_cast<const uint8_t*>(in) + static_cast<size_t>(c->d.rank) * bytes;
+  if (!in_place && overlaps(out, bytes, in, static_cast<size_t>(W) * bytes))
     return fail(B2_EINVAL, "b2_reduce_scatter: `out` overlaps `in` other than as this rank's block");
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (W == 1) {
-    if (o != own) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
+    if (!in_place) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
     return B2_OK;
   }
   const bool sum = !dtype_is_int(dtype) && (op == B2_OP_SUM || op == B2_OP_AVG);
@@ -1483,27 +1482,24 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
   const float scale = op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f;
   uint8_t* po = static_cast<uint8_t*>(out);
   const uint8_t* pi = static_cast<const uint8_t*>(in);
-  size_t off = 0;
-  while (off < n_elems) {
-    const size_t n = n_elems - off < cap ? n_elems - off : cap;
-    cudaError_t e = cudaErrorInvalidValue;  // never guess a mode
+  const cudaError_t e = for_chunks(c, n_elems, cap, [&](size_t off, size_t n) {
+    cudaError_t le = cudaErrorInvalidValue;  // never guess a mode
     if (sum) {
       const int grid = grid_for(c, (n + 7) / 8, vecs_per_trip(W));
       with_mode(mode, [&](auto m) {
-        e = launch_reduce_scatter<decltype(m)::value>(c->d, kNoSrc, grid, po + off * eb, pi + off * eb, n, n_elems, scale, s);
+        le = launch_reduce_scatter<decltype(m)::value>(c->d, kNoSrc, grid, po + off * eb, pi + off * eb, n, n_elems, scale, s);
       });
     } else {
       const int grid = grid_for(c, (n * eb + 15) / 16, 1);
       with_exact_op(dtype, op, [&](auto dt, auto oc) {
         k_reduce_scatter_exact<decltype(dt)::value, decltype(oc)::value><<<grid, kThreads, 0, s>>>(c->d, po + off * eb, pi + off * eb,
                                                                                                  n, n_elems);
-        e = cudaGetLastError();
+        le = cudaGetLastError();
       });
     }
-    if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
-    c->launches++;
-    off += n;
-  }
+    return le;
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -1518,15 +1514,11 @@ int b2_alltoall(b2_comm_t* c, void* const* out, const size_t* recv_bytes, const 
     if (!out[r] && recv_bytes[r]) return fail(B2_EINVAL, "b2_alltoall: out[%d] is null but recv_bytes[%d] = %zu", r, r, recv_bytes[r]);
     if (!in[r] && send_bytes[r]) return fail(B2_EINVAL, "b2_alltoall: in[%d] is null but send_bytes[%d] = %zu", r, r, send_bytes[r]);
   }
-  const auto overlap = [](const void* p, size_t n, const void* q, size_t m) {
-    const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
-    return n && m && a < b + m && b < a + n;
-  };
   for (int r = 0; r < W; ++r) {
     for (int s = r + 1; s < W; ++s)
-      if (overlap(out[r], recv_bytes[r], out[s], recv_bytes[s])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps out[%d]", r, s);
+      if (overlaps(out[r], recv_bytes[r], out[s], recv_bytes[s])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps out[%d]", r, s);
     for (int j = 0; j < W; ++j)
-      if (overlap(out[r], recv_bytes[r], in[j], send_bytes[j])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps in[%d]", r, j);
+      if (overlaps(out[r], recv_bytes[r], in[j], send_bytes[j])) return fail(B2_EINVAL, "b2_alltoall: out[%d] overlaps in[%d]", r, j);
   }
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
@@ -1573,13 +1565,10 @@ int b2_p2p(b2_comm_t* c, const b2_p2p_op_t* ops, int n_ops, void* stream) {
     if (!ops[i].ptr && ops[i].bytes) return fail(B2_EINVAL, "b2_p2p: op %d has a null pointer and %zu bytes", i, ops[i].bytes);
   }
   for (int i = 0; i < n_ops; ++i) {
-    if (ops[i].is_send || !ops[i].bytes) continue;
-    const uintptr_t a = reinterpret_cast<uintptr_t>(ops[i].ptr);
-    for (int j = 0; j < n_ops; ++j) {
-      const uintptr_t b = reinterpret_cast<uintptr_t>(ops[j].ptr);
-      if (j != i && ops[j].bytes && a < b + ops[j].bytes && b < a + ops[i].bytes)
+    if (ops[i].is_send) continue;
+    for (int j = 0; j < n_ops; ++j)
+      if (j != i && overlaps(ops[i].ptr, ops[i].bytes, ops[j].ptr, ops[j].bytes))
         return fail(B2_EINVAL, "b2_p2p: op %d (a recv) overlaps op %d", i, j);
-    }
   }
   if (const int rc = check_not_poisoned(c)) return rc;
   // Channels in order of first appearance; an op's chunks follow the chunks of the earlier ops on its channel.

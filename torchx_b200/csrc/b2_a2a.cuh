@@ -41,7 +41,7 @@ constexpr size_t kA2aHeaderBytes = 16;  // at the start of every recv region; a 
 __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) {
   using namespace dev;
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
   const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
 
@@ -68,9 +68,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) 
 #pragma unroll
   for (int jj = 1; jj < B2_MAX_WORLD; ++jj) {
     if (jj < c.world) {
-      int r = c.rank + jj;  // the rank whose region this is
-      if (r >= c.world) r -= c.world;
-      const uint4 h = ldg_u4(mine + r * c.slice_cap);
+      const uint4 h = ldg_u4(mine + rank_at(c, jj) * c.slice_cap);  // the header of rank (rank + jj) % world
       const unsigned long long count = (static_cast<unsigned long long>(h.y) << 32) | h.x;
       ok = ok && h.z == 0 && count == a.recv_bytes[jj];
     }
@@ -79,8 +77,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) 
 #pragma unroll
     for (int jj = 0; jj < B2_MAX_WORLD; ++jj) {
       if (jj < c.world) {
-        int r = c.rank + jj;
-        if (r >= c.world) r -= c.world;
+        const int r = rank_at(c, jj);
         const unsigned long long n = a.recv_bytes[jj];
         uint8_t* dst = a.recv[jj];
         const bool dst_aligned = (reinterpret_cast<uintptr_t>(dst) & 15u) == 0;
@@ -93,8 +90,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) 
       }
     }
   } else if (blockIdx.x == 0 && threadIdx.x == 0 && ld_volatile_u32(c.status) == 0) {  // a timeout recorded first stays
-    *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_EINVAL);
-    __threadfence_system();
+    record_status(c.status, B2_EINVAL);
   }
   op_end(c, seq0);
 }

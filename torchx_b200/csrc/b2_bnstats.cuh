@@ -54,7 +54,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   const uint8_t* mine = nullptr;
   if (!solo) {
     seq0 = op_begin(c);
-    const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+    const unsigned long long stage = stage_of(c, seq0);
     for (unsigned long long v = threadIdx.x; v <= 2 * Cv; v += kThreads) {
       uint4 q;
       if (v < Cv) q = exact::ld_local<4>(pm, am, v, C);

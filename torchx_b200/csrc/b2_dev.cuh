@@ -644,10 +644,17 @@ __device__ __forceinline__ int slice_of(int rank, int jj) {
   return j;
 }
 
-// A peer wait gave up: record it in the host-mapped status word (b2_comm_status).  Results are undefined from here on,
-// but the GPU is not hung.
-__device__ __forceinline__ void record_timeout(const CommDev& c) {
-  *reinterpret_cast<volatile uint32_t*>(c.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
+// slice_of for the kernels that take the world size at run time (jj < W).
+__device__ __forceinline__ int rank_at(const CommDev& c, int jj) {
+  int r = c.rank + jj;
+  if (r >= c.world) r -= c.world;
+  return r;
+}
+
+// Record B2_E* `code` in the host-mapped status word (b2_comm_status): B2_ETIMEOUT when a peer wait gave up (results are
+// undefined from here on, but the GPU is not hung), B2_EINVAL when ranks disagreed on sizes.
+__device__ __forceinline__ void record_status(uint32_t* status, int code) {
+  *reinterpret_cast<volatile uint32_t*>(status) = static_cast<uint32_t>(-code);
   __threadfence_system();
 }
 
@@ -663,7 +670,7 @@ __device__ __forceinline__ void wait_flag(const CommDev& c, const uint32_t* flag
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > c.timeout_ns) {
-        record_timeout(c);
+        record_status(c.status, B2_ETIMEOUT);
         break;
       }
     }
@@ -686,7 +693,7 @@ __device__ __forceinline__ void wait_wire(const CommDev& c, const uint8_t* p, Wi
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > c.timeout_ns) {
-        record_timeout(c);
+        record_status(c.status, B2_ETIMEOUT);
         break;
       }
     }
@@ -700,8 +707,7 @@ __device__ __forceinline__ void cta_xbar(const CommDev& c, uint32_t seq) {
   __syncthreads();  // all of this CTA's data stores are ordered before the release below
   if (threadIdx.x < c.world) {
     const int jj = threadIdx.x;  // this thread pairs with rank p = (rank + jj) % world
-    int p = c.rank + jj;
-    if (p >= c.world) p -= c.world;
+    const int p = rank_at(c, jj);
     const size_t slot = c.flag_off + static_cast<size_t>(blockIdx.x) * kFlagSlotBytes;
     uint32_t* theirs = reinterpret_cast<uint32_t*>(peer_sel(c, jj) + slot) + c.rank;
     const uint32_t* mine = reinterpret_cast<const uint32_t*>(c.peer[0] + slot) + p;
@@ -716,6 +722,11 @@ __device__ __forceinline__ void cta_xbar(const CommDev& c, uint32_t seq) {
 // all CTAs are through.  Keeping the counter on the device makes the launch sequence CUDA-graph
 // replayable and keeps the host stateless.
 __device__ __forceinline__ uint32_t op_begin(const CommDev& c) { return ld_volatile_u32(c.opseq); }
+
+// The staging buffer of the op whose counter is seq0: consecutive ops alternate between the two.
+__device__ __forceinline__ unsigned long long stage_of(const CommDev& c, uint32_t seq0) {
+  return (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+}
 
 __device__ __forceinline__ void op_end(const CommDev& c, uint32_t seq0) {
   __syncthreads();

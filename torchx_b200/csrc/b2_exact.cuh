@@ -13,33 +13,38 @@
 
 namespace exact {
 
-// Element size and kind of each B2_DT_* (include/b200ddp.h).
+// Name (as torch spells it), element size and kind of each B2_DT_* (include/b200ddp.h).
 template <int DT>
 struct DtypeTraits {
   static_assert(DT < 0 && DT >= 0, "unknown B2 dtype: add its DtypeTraits specialisation");
 };
 template <>
 struct DtypeTraits<B2_DT_INT32> {
+  static constexpr const char* kName = "int32";
   static constexpr int kBytes = 4;
   static constexpr bool kInt = true;
 };
 template <>
 struct DtypeTraits<B2_DT_INT64> {
+  static constexpr const char* kName = "int64";
   static constexpr int kBytes = 8;
   static constexpr bool kInt = true;
 };
 template <>
 struct DtypeTraits<B2_DT_FLOAT32> {
+  static constexpr const char* kName = "float32";
   static constexpr int kBytes = 4;
   static constexpr bool kInt = false;
 };
 template <>
 struct DtypeTraits<B2_DT_BFLOAT16> {
+  static constexpr const char* kName = "bfloat16";
   static constexpr int kBytes = 2;
   static constexpr bool kInt = false;
 };
 template <>
 struct DtypeTraits<B2_DT_FLOAT16> {
+  static constexpr const char* kName = "float16";
   static constexpr int kBytes = 2;
   static constexpr bool kInt = false;
 };
@@ -200,7 +205,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_exact(CommDev c, void* b
   using namespace dev;
   constexpr int E = exact::DtypeTraits<DT>::kBytes;
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   uint8_t* p = static_cast<uint8_t*>(buf);
   const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
   const unsigned long long V = (n * E + 15) / 16;
@@ -229,7 +234,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     k_allgather(CommDev c, uint8_t* out, const uint8_t* in, unsigned long long bytes, unsigned long long block) {
   using namespace dev;
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const bool in_aligned = (reinterpret_cast<uintptr_t>(in) & 15u) == 0;
   const bool in_place = in == out + static_cast<unsigned long long>(c.rank) * block;
   const unsigned long long V = (bytes + 15) / 16;

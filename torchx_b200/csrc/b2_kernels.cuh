@@ -223,7 +223,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
@@ -293,7 +293,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long Ls = (V + W - 1) / W;
@@ -397,7 +397,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     k_broadcast(CommDev c, uint8_t* buf, unsigned long long bytes, int root) {
   using namespace dev;
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
   const unsigned long long nvec = bytes / 16;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;

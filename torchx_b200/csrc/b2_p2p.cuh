@@ -96,8 +96,7 @@ __device__ __forceinline__ bool wait(const P2pArgs& a, const uint32_t* flag, uin
       if (t0 == 0) {
         t0 = now;
       } else if (now - t0 > a.timeout_ns) {
-        *reinterpret_cast<volatile uint32_t*>(a.status) = static_cast<uint32_t>(-B2_ETIMEOUT);
-        __threadfence_system();
+        dev::record_status(a.status, B2_ETIMEOUT);
         return false;
       }
     }
@@ -145,8 +144,7 @@ __device__ __forceinline__ void recv_chunk(const P2pArgs& a, const P2pChan& ch, 
   } else if (threadIdx.x == 0 && dev::ld_volatile_u32(a.status) == 0) {
     reinterpret_cast<volatile uint32_t*>(a.status)[1] = kStatusP2p;
     __threadfence_system();
-    *reinterpret_cast<volatile uint32_t*>(a.status) = static_cast<uint32_t>(-B2_EINVAL);
-    __threadfence_system();
+    dev::record_status(a.status, B2_EINVAL);
   }
   __syncthreads();  // every thread's loads of the slot are ordered before the release below
   if (threadIdx.x == 0) dev::st_release_sys(ch.credit + slot * kP2pLineWords, n + 1u);

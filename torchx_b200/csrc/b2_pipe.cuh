@@ -125,7 +125,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   __shared__ uint32_t mail[2];  // [0]: chunks role A has finished, [1]: chunks role B has finished
   const uint32_t seq0 = op_begin(c);
   const uint32_t seq = seq0 * 4u + 1u;
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long Ls = (V + W - 1) / W;

@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
   const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
@@ -108,6 +108,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int WVB = Wire<MODE>::kBytes;
   __shared__ OptCta t;
   const uint32_t seq0 = op_begin(c);
+  // stage_of(c, seq0), open-coded: the call moves ptxas's register allocation of 8 instances (modes 0, 1 and 3 at W <= 4)
   const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
@@ -137,7 +138,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter_exact(CommDev c,
   using namespace dev;
   constexpr int E = exact::DtypeTraits<DT>::kBytes;
   const uint32_t seq0 = op_begin(c);
-  const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
+  const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long V = (n * E + 15) / 16;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
   const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
@@ -147,9 +148,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter_exact(CommDev c,
 #pragma unroll
     for (int jj = 0; jj < B2_MAX_WORLD; ++jj) {
       if (jj < c.world) {
-        int j = c.rank + jj;  // the rank whose block goes to peer[jj]
-        if (j >= c.world) j -= c.world;
-        const uint8_t* src = static_cast<const uint8_t*>(in) + j * block * E;
+        const uint8_t* src = static_cast<const uint8_t*>(in) + rank_at(c, jj) * block * E;  // the block that goes to peer[jj]
         q[jj] = exact::ld_local<E>(src, (reinterpret_cast<uintptr_t>(src) & 15u) == 0, v, n);
       }
     }

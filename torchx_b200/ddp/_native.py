@@ -67,48 +67,6 @@ NVCC_FLAGS = [
     "-shared",
 ]
 
-# every symbol include/b200ddp.h declares (tests/test_abi.py checks the header and this list agree)
-SYMBOLS = [
-    "b2_version",
-    "b2_last_error",
-    "b2_comm_create",
-    "b2_comm_create_local",
-    "b2_comm_destroy",
-    "b2_comm_rank",
-    "b2_comm_world",
-    "b2_comm_device",
-    "b2_comm_caps",
-    "b2_comm_set_timeout_ms",
-    "b2_comm_set_max_ctas",
-    "b2_comm_set_param",
-    "b2_comm_status",
-    "b2_comm_launch_count",
-    "b2_comm_last_algo",
-    "b2_auto_algo",
-    "b2_comm_trace",
-    "b2_allreduce",
-    "b2_allreduce_gather",
-    "b2_broadcast",
-    "b2_allreduce_op",
-    "b2_allgather",
-    "b2_reduce_scatter",
-    "b2_reduce_scatter_gather",
-    "b2_reduce_scatter_step",
-    "b2_alltoall",
-    "b2_alltoall_max_bytes",
-    "b2_p2p",
-    "b2_p2p_eager_bytes",
-    "b2_batchnorm_stats",
-    "b2_bn_forward_elemt",
-    "b2_bn_backward_elemt",
-    "b2_bn_reduce_plan",
-    "b2_bn_stats",
-    "b2_bn_backward_reduce",
-    "b2_barrier",
-    "b2_local_pass",
-]
-
-
 B2_MAX_SEGMENTS = 128
 
 
@@ -153,6 +111,52 @@ class B2Optim(ctypes.Structure):
                 ("run_scalar", ctypes.c_uint8 * B2_OPT_MAX_RUNS), ("group", B2OptimGroup * B2_OPT_MAX_GROUPS)]
 
 
+_vp, _i, _sz, _u64, _f, _d = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_uint64, ctypes.c_float, ctypes.c_double
+_P = ctypes.POINTER
+
+# name -> (restype, argtypes) of every symbol include/b200ddp.h declares (tests/test_abi.py checks the header and SYMBOLS agree)
+SIGNATURES = {
+    "b2_version": (_i, []),
+    "b2_last_error": (ctypes.c_char_p, []),
+    "b2_comm_create": (_i, [_P(_vp), _i, _i, _i, ctypes.c_char_p, _u64, _sz, _i]),
+    "b2_comm_create_local": (_i, [_P(_vp), _i, _P(_i), _sz]),
+    "b2_comm_destroy": (_i, [_vp]),
+    "b2_comm_rank": (_i, [_vp]),
+    "b2_comm_world": (_i, [_vp]),
+    "b2_comm_device": (_i, [_vp]),
+    "b2_comm_caps": (_i, [_vp]),
+    "b2_comm_set_timeout_ms": (_i, [_vp, _i]),
+    "b2_comm_set_max_ctas": (_i, [_vp, _i]),
+    "b2_comm_set_param": (_i, [_vp, ctypes.c_char_p, ctypes.c_longlong]),
+    "b2_comm_status": (_i, [_vp]),
+    "b2_comm_launch_count": (_u64, [_vp]),
+    "b2_comm_last_algo": (_i, [_vp]),
+    "b2_auto_algo": (_i, [_i, _i, _sz, _i]),
+    "b2_comm_trace": (_i, [_vp, _i, _P(_u64), _i]),
+    "b2_allreduce": (_i, [_vp, _vp, _sz, _i, _f, _i, _vp]),
+    "b2_allreduce_gather": (_i, [_vp, _vp, _sz, _P(B2Segment), _i, _i, _f, _i, _vp]),
+    "b2_broadcast": (_i, [_vp, _vp, _sz, _i, _vp]),
+    "b2_allreduce_op": (_i, [_vp, _vp, _sz, _i, _i, _vp]),
+    "b2_allgather": (_i, [_vp, _vp, _vp, _sz, _vp]),
+    "b2_reduce_scatter": (_i, [_vp, _vp, _vp, _sz, _i, _i, _vp]),
+    "b2_reduce_scatter_gather": (_i, [_vp, _vp, _sz, _P(B2Segment), _i, _i, _f, _vp]),
+    "b2_reduce_scatter_step": (_i, [_vp, _sz, _P(B2Segment), _i, _i, _f, _P(B2Optim), _vp]),
+    "b2_alltoall": (_i, [_vp, _P(_vp), _P(_sz), _P(_vp), _P(_sz), _vp]),
+    "b2_alltoall_max_bytes": (_sz, [_vp]),
+    "b2_p2p": (_i, [_vp, _P(B2P2pOp), _i, _vp]),
+    "b2_p2p_eager_bytes": (_sz, [_vp]),
+    "b2_batchnorm_stats": (_i, [_vp, _vp, _vp, _f, _sz, _vp, _vp, _d, _d, _vp, _vp]),
+    "b2_bn_forward_elemt": (_i, [_vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _d, _vp, _i, _vp]),
+    "b2_bn_backward_elemt": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    "b2_bn_reduce_plan": (_i, [_sz, _sz, _P(_i), _P(_sz)]),
+    "b2_bn_stats": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _d, _vp, _sz, _i, _vp]),
+    "b2_bn_backward_reduce": (_i, [_vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
+    "b2_barrier": (_i, [_vp, _vp]),
+    "b2_local_pass": (_i, [_vp, _sz, _i, _f, _i, _vp]),
+}
+SYMBOLS = list(SIGNATURES)
+
+
 class B2Error(RuntimeError):
     def __init__(self, code: int, msg: str) -> None:
         super().__init__(f"libb200ddp error {code}: {msg}")
@@ -190,72 +194,10 @@ def lib() -> ctypes.CDLL:
             "`python -c 'import __graft_entry__ as g; g.build()'` (needs nvcc). There is no CPU fallback."
         )
     L = ctypes.CDLL(LIB_PATH)
-    vp, i, sz, u64, f = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_uint64, ctypes.c_float
-    L.b2_version.restype = i
-    L.b2_version.argtypes = []
-    L.b2_last_error.restype = ctypes.c_char_p
-    L.b2_last_error.argtypes = []
-    L.b2_comm_create.restype = i
-    L.b2_comm_create.argtypes = [ctypes.POINTER(vp), i, i, i, ctypes.c_char_p, u64, sz, i]
-    L.b2_comm_create_local.restype = i
-    L.b2_comm_create_local.argtypes = [ctypes.POINTER(vp), i, ctypes.POINTER(i), sz]
-    L.b2_comm_destroy.restype = i
-    L.b2_comm_destroy.argtypes = [vp]
-    for name in ("b2_comm_rank", "b2_comm_world", "b2_comm_device", "b2_comm_status", "b2_comm_caps", "b2_comm_last_algo"):
-        getattr(L, name).restype = i
-        getattr(L, name).argtypes = [vp]
-    L.b2_comm_set_timeout_ms.restype = i
-    L.b2_comm_set_timeout_ms.argtypes = [vp, i]
-    L.b2_comm_set_max_ctas.restype = i
-    L.b2_comm_set_max_ctas.argtypes = [vp, i]
-    L.b2_comm_set_param.restype = i
-    L.b2_comm_set_param.argtypes = [vp, ctypes.c_char_p, ctypes.c_longlong]
-    L.b2_auto_algo.restype = i
-    L.b2_auto_algo.argtypes = [i, i, sz, i]
-    L.b2_comm_launch_count.restype = u64
-    L.b2_comm_launch_count.argtypes = [vp]
-    L.b2_comm_trace.restype = i
-    L.b2_comm_trace.argtypes = [vp, i, ctypes.POINTER(u64), i]
-    L.b2_allreduce.restype = i
-    L.b2_allreduce.argtypes = [vp, vp, sz, i, f, i, vp]
-    L.b2_allreduce_gather.restype = i
-    L.b2_allreduce_gather.argtypes = [vp, vp, sz, ctypes.POINTER(B2Segment), i, i, f, i, vp]
-    L.b2_broadcast.restype = i
-    L.b2_broadcast.argtypes = [vp, vp, sz, i, vp]
-    L.b2_allreduce_op.restype = i
-    L.b2_allreduce_op.argtypes = [vp, vp, sz, i, i, vp]
-    L.b2_allgather.restype = i
-    L.b2_allgather.argtypes = [vp, vp, vp, sz, vp]
-    L.b2_reduce_scatter.restype = i
-    L.b2_reduce_scatter.argtypes = [vp, vp, vp, sz, i, i, vp]
-    L.b2_reduce_scatter_gather.restype = i
-    L.b2_reduce_scatter_gather.argtypes = [vp, vp, sz, ctypes.POINTER(B2Segment), i, i, f, vp]
-    L.b2_reduce_scatter_step.restype = i
-    L.b2_reduce_scatter_step.argtypes = [vp, sz, ctypes.POINTER(B2Segment), i, i, f, ctypes.POINTER(B2Optim), vp]
-    L.b2_alltoall.restype = i
-    L.b2_alltoall.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(sz), ctypes.POINTER(vp), ctypes.POINTER(sz), vp]
-    L.b2_alltoall_max_bytes.restype = sz
-    L.b2_alltoall_max_bytes.argtypes = [vp]
-    L.b2_p2p.restype = i
-    L.b2_p2p.argtypes = [vp, ctypes.POINTER(B2P2pOp), i, vp]
-    L.b2_p2p_eager_bytes.restype = sz
-    L.b2_p2p_eager_bytes.argtypes = [vp]
-    L.b2_batchnorm_stats.restype = i
-    L.b2_batchnorm_stats.argtypes = [vp, vp, vp, f, sz, vp, vp, ctypes.c_double, ctypes.c_double, vp, vp]
-    L.b2_bn_forward_elemt.restype = i
-    L.b2_bn_forward_elemt.argtypes = [vp, vp, sz, sz, i, vp, vp, vp, vp, ctypes.c_double, vp, i, vp]
-    L.b2_bn_backward_elemt.restype = i
-    L.b2_bn_backward_elemt.argtypes = [vp, vp, vp, sz, sz, i, vp, vp, vp, vp, vp, i, vp]
-    L.b2_bn_reduce_plan.restype = i
-    L.b2_bn_reduce_plan.argtypes = [sz, sz, ctypes.POINTER(i), ctypes.POINTER(sz)]
-    L.b2_bn_stats.restype = i
-    L.b2_bn_stats.argtypes = [vp, sz, sz, i, vp, vp, vp, vp, ctypes.c_double, vp, sz, i, vp]
-    L.b2_bn_backward_reduce.restype = i
-    L.b2_bn_backward_reduce.argtypes = [vp, vp, sz, sz, i, vp, vp, vp, vp, vp, vp, vp, sz, i, vp]
-    L.b2_barrier.restype = i
-    L.b2_barrier.argtypes = [vp, vp]
-    L.b2_local_pass.restype = i
-    L.b2_local_pass.argtypes = [vp, sz, i, f, i, vp]
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype = restype
+        fn.argtypes = argtypes
     if L.b2_version() != B2_ABI_VERSION:
         raise ImportError(f"libb200ddp ABI {L.b2_version()} != binding {B2_ABI_VERSION}; rebuild")
     _lib = L

@@ -69,9 +69,10 @@ def as_rank(x) -> Optional[int]:
         return None
 
 
-def _stream_ptr(stream: Optional[torch.cuda.Stream], device: int) -> int:
+def _stream_arg(stream: Optional[torch.cuda.Stream], device: int) -> ctypes.c_void_p:
+    """The cudaStream_t argument of a library call: ``stream``, or the device's current stream."""
     s = stream if stream is not None else torch.cuda.current_stream(device)
-    return int(s.cuda_stream)
+    return ctypes.c_void_p(s.cuda_stream)
 
 
 def default_shm_name() -> str:
@@ -201,10 +202,8 @@ class Communicator:
                    stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
         """In-place ``t <- round(sum_r wire(scale * t_r))``; scale defaults to 1/world (gradient averaging)."""
         self._check_tensor(t)
-        if scale is None:
-            scale = 1.0 / self.world
         N.check(N.lib().b2_allreduce(self._h, ctypes.c_void_p(t.data_ptr()), t.numel(), mode_for(t, wire),
-                                     ctypes.c_float(scale), ALGOS[algo], ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                     self._scale(scale), ALGOS[algo], _stream_arg(stream, self.device)))
         return t
 
     def allreduce_gather_(self, out: torch.Tensor, segments, n_segments: int, scale: Optional[float] = None, wire: str = "bf16",
@@ -214,16 +213,14 @@ class Communicator:
         ctypes array of ``_native.B2Segment`` (device pointer, begin, end) covering the bucket in order; it is copied into
         the kernel parameters by the call."""
         self._check_tensor(out)
-        if scale is None:
-            scale = 1.0 / self.world
         N.check(N.lib().b2_allreduce_gather(self._h, ctypes.c_void_p(out.data_ptr()), out.numel(), segments, n_segments, mode_for(out, wire),
-                                            ctypes.c_float(scale), ALGOS[algo], ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                            self._scale(scale), ALGOS[algo], _stream_arg(stream, self.device)))
         return out
 
     def broadcast_(self, t: torch.Tensor, root: int = 0, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
         self._check_tensor(t)
         N.check(N.lib().b2_broadcast(self._h, ctypes.c_void_p(t.data_ptr()), t.numel() * t.element_size(), root,
-                                     ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                     _stream_arg(stream, self.device)))
         return t
 
     def allreduce_op_(self, t: torch.Tensor, op: str = "sum", stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
@@ -232,7 +229,7 @@ class Communicator:
         dt, code = dtype_op_for(t.dtype, op)
         self._check_tensor(t)
         N.check(N.lib().b2_allreduce_op(self._h, ctypes.c_void_p(t.data_ptr()), t.numel(), dt, code,
-                                        ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                        _stream_arg(stream, self.device)))
         return t
 
     def allgather_(self, out: torch.Tensor, t: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
@@ -245,7 +242,7 @@ class Communicator:
         if out.numel() != self.world * t.numel():
             raise ValueError(f"allgather_: out has {out.numel()} elements, needs {self.world} x {t.numel()}")
         N.check(N.lib().b2_allgather(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()),
-                                     t.numel() * t.element_size(), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                     t.numel() * t.element_size(), _stream_arg(stream, self.device)))
         return out
 
     def reduce_scatter_(self, out: torch.Tensor, t: torch.Tensor, op: str = "sum",
@@ -261,7 +258,7 @@ class Communicator:
         self._check_tensor(out)
         self._check_tensor(t)
         N.check(N.lib().b2_reduce_scatter(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()), out.numel(), dt,
-                                          code, ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                          code, _stream_arg(stream, self.device)))
         return out
 
     def reduce_scatter_gather_(self, out: torch.Tensor, segments, n_segments: int, scale: Optional[float] = None,
@@ -271,11 +268,9 @@ class Communicator:
         there wherever it sums in rank order, moving only (W-1)/W of the wire data.  The gradient shard of the sharded
         mini-DDP."""
         self._check_tensor(out)
-        if scale is None:
-            scale = 1.0 / self.world
         N.check(N.lib().b2_reduce_scatter_gather(self._h, ctypes.c_void_p(out.data_ptr()), out.numel(), segments, n_segments,
-                                                 mode_for(out, wire), ctypes.c_float(scale),
-                                                 ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                                 mode_for(out, wire), self._scale(scale),
+                                                 _stream_arg(stream, self.device)))
         return out
 
     def reduce_scatter_step_(self, block: int, segments, n_segments: int, opt, scale: Optional[float] = None,
@@ -284,13 +279,11 @@ class Communicator:
         reduced block steps this rank's block of the flat fp32 parameter buffer and its optimizer state as ``opt`` (a
         ``_native.B2Optim``) describes them, with the arithmetic of torch's fused SGD / Adam / AdamW.  The overlap mode of
         the sharded mini-DDP."""
-        if scale is None:
-            scale = 1.0 / self.world
         mode = _MODE_FOR.get(("f32", wire))
         if mode is None:
             raise ValueError(f"unsupported wire format {wire!r}")
-        N.check(N.lib().b2_reduce_scatter_step(self._h, block, segments, n_segments, mode, ctypes.c_float(scale),
-                                               ctypes.byref(opt), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        N.check(N.lib().b2_reduce_scatter_step(self._h, block, segments, n_segments, mode, self._scale(scale),
+                                               ctypes.byref(opt), _stream_arg(stream, self.device)))
 
     def alltoall_(self, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor],
                   stream: Optional[torch.cuda.Stream] = None) -> Sequence[torch.Tensor]:
@@ -313,7 +306,7 @@ class Communicator:
             return (ctypes.c_size_t * self.world)(*(t.numel() * t.element_size() for t in ts))
 
         N.check(N.lib().b2_alltoall(self._h, ptrs(outs), sizes(outs), ptrs(ins), sizes(ins),
-                                    ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                    _stream_arg(stream, self.device)))
         return outs
 
     def p2p_(self, ops: Sequence, stream: Optional[torch.cuda.Stream] = None) -> None:
@@ -336,7 +329,7 @@ class Communicator:
         for k, ((kind, t, _), peer) in enumerate(zip(ops, peers)):
             self._check_tensor(t)
             arr[k] = N.B2P2pOp(peer, int(kind == "send"), t.data_ptr(), t.numel() * t.element_size())
-        N.check(N.lib().b2_p2p(self._h, arr, len(ops), ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        N.check(N.lib().b2_p2p(self._h, arr, len(ops), _stream_arg(stream, self.device)))
 
     def batchnorm_stats_(self, mean: torch.Tensor, invstd: torch.Tensor, count: float, running_mean: Optional[torch.Tensor] = None,
                          running_var: Optional[torch.Tensor] = None, *, momentum: float, eps: float,
@@ -362,10 +355,14 @@ class Communicator:
 
         N.check(N.lib().b2_batchnorm_stats(self._h, ptr(mean), ptr(invstd), ctypes.c_float(count), C, ptr(running_mean),
                                            ptr(running_var), float(momentum), float(eps), ptr(counts_out),
-                                           ctypes.c_void_p(_stream_ptr(stream, self.device))))
+                                           _stream_arg(stream, self.device)))
 
     def barrier(self, stream: Optional[torch.cuda.Stream] = None) -> None:
-        N.check(N.lib().b2_barrier(self._h, ctypes.c_void_p(_stream_ptr(stream, self.device))))
+        N.check(N.lib().b2_barrier(self._h, _stream_arg(stream, self.device)))
+
+    def _scale(self, scale: Optional[float]) -> ctypes.c_float:
+        """The scale argument of a gradient collective: 1/world (gradient averaging) unless given."""
+        return ctypes.c_float(1.0 / self.world if scale is None else scale)
 
     def _check_tensor(self, t: torch.Tensor) -> None:
         if not t.is_cuda or t.device.index != self.device:
@@ -378,5 +375,5 @@ def local_pass_(t: torch.Tensor, scale: float = 1.0, wire: str = "bf16", stream:
     """The W == 1 fused cast/scale pass (b2_local_pass) on its own."""
     dev = t.device.index
     N.check(N.lib().b2_local_pass(ctypes.c_void_p(t.data_ptr()), t.numel(), mode_for(t, wire), ctypes.c_float(scale), dev,
-                                  ctypes.c_void_p(_stream_ptr(stream, dev))))
+                                  _stream_arg(stream, dev)))
     return t
