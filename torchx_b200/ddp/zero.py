@@ -8,8 +8,9 @@ This one runs on the native communicator instead:
   * ``step()`` steps the inner optimizer on this rank's slice of the parameters only, then all-gathers every bucket's
     flat parameter buffer in place (exact bytes).
 
-SGD, Adam and AdamW are elementwise, so stepping a slice gives the bits of stepping the whole tensor: the parameters
-stay bit-equal to those of the unsharded mini-DDP under the same optimizer, and the consolidated state to its state.
+SGD, Adam and AdamW are elementwise, so stepping a slice gives the bits of stepping the whole tensor, with two exceptions
+in torch's fused kernels (DESIGN.md 2.4) that the constructor refuses where they would apply: the parameters stay
+bit-equal to those of the unsharded mini-DDP under the same optimizer, and the consolidated state to its state.
 """
 from __future__ import annotations
 
@@ -20,7 +21,8 @@ import torch
 from . import _native as N
 from .ddp import DistributedDataParallel, _view_like
 
-# the elementwise optimizers: a slice of a tensor steps to the bits of the same slice of the stepped tensor
+# the elementwise optimizers: a slice of a tensor steps to the bits of the same slice of the stepped tensor (two fused
+# exceptions: _check_split_params)
 SUPPORTED = (torch.optim.SGD, torch.optim.Adam, torch.optim.AdamW)
 
 
@@ -122,6 +124,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             _check_run_bound([[gi_of[id(p)] for p in b.params] for b in model.buckets],
                              [[0] * len(b.params) for b in model.buckets], optimizer_class is torch.optim.SGD,
                              [[pos[gi_of[id(p)]] for p in b.params] for b in model.buckets])
+        else:
+            _check_split_params(optimizer_class, groups, defaults, model)
         super().__init__(groups, defaults)  # validates the groups and fills in the defaults
         self.model = model
         self.comm = model.comm
@@ -506,6 +510,43 @@ def _check_overlap(groups: List[Dict[str, Any]], defaults: Dict[str, Any], model
         for k in ("capturable", "differentiable"):
             if opts.get(k):
                 raise ValueError(f"overlap_with_ddp=True does not support {k}=True")
+
+
+def _check_split_params(optimizer_class: type, groups: List[Dict[str, Any]], defaults: Dict[str, Any],
+                        model: DistributedDataParallel) -> None:
+    """Without overlap the inner optimizer steps one 1-D view per (parameter, rank block).  Two of torch's fused kernels do
+    not step such views to the bits of the whole tensor when a block boundary splits a parameter of a numel that is not a
+    multiple of 4 (the whole tensor takes their scalar path, a view of a multiple of 4 elements the vectorised one, and a
+    view counts its elements from 0; DESIGN.md 2.4): Adam with coupled weight decay and without maximize, whose rounding of
+    ``param * weight_decay`` depends on an element's index, and SGD with maximize, momentum and no weight decay, whose
+    momentum update is contracted differently on the two paths.  Refused here, from the bucket layout alone, so every rank
+    raises alike before anything is sharded."""
+    W = model.world_size
+    names = {id(p): n for n, p in model.module.named_parameters()}
+    gi_of = {id(p): gi for gi, g in enumerate(groups) for p in g["params"]}
+    what = []
+    for g in groups:
+        o = {**defaults, **g}
+        if not o.get("fused"):
+            what.append(None)
+        elif optimizer_class is torch.optim.Adam and o.get("weight_decay", 0) and not o.get("maximize"):
+            what.append("Adam(fused=True) with weight_decay")
+        elif (optimizer_class is torch.optim.SGD and o.get("maximize") and o.get("momentum", 0)
+              and not o.get("weight_decay", 0)):
+            what.append("SGD(fused=True) with maximize, momentum and no weight_decay")
+        else:
+            what.append(None)
+    for b in model.buckets:
+        B = padded_block(b.spec.numel, W)
+        for p, off, n in zip(b.params, b.spec.offsets, b.spec.numels):
+            w = what[gi_of[id(p)]]
+            if w is None or n % 4 == 0 or off // B == (off + n - 1) // B:
+                continue
+            fix = ("overlap_with_ddp=True (whose fused step is exact here) or foreach=True" if optimizer_class is torch.optim.Adam
+                   else "foreach=True")
+            raise ValueError(
+                f"ZeroRedundancyOptimizer: parameter {names.get(id(p), '?')!r} ({n} elements, not a multiple of 4) is split "
+                f"between rank blocks, and {w} would step its pieces to other bits than the whole tensor; use {fix}")
 
 
 def _owns(where, rank: int) -> bool:
