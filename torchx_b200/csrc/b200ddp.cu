@@ -1768,13 +1768,11 @@ int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* m
   const float mom = static_cast<float>(momentum);
   const float bessel = static_cast<float>(static_cast<double>(rows) / static_cast<double>(rows - 1));
   float* ws = static_cast<float*>(workspace);
-  const int vw = bn::reduce_vecs(t, C);
-  k_bn2d_stats<kBnStatsUnroll><<<dim3((C / 8 + vw - 1) / vw, t.grid_y), vw * t.block_y * bn::kAtenLoads, 0, s>>>(
-      static_cast<const uint16_t*>(x), M, C, t, vw, mean, var, running_mean, running_var, mom, bessel, ws);
-  if (t.grid_y > 1) {
-    const int mw = bn::merge_vecs(t, C);
-    k_bn2d_stats_merge<<<(C / 8 + mw - 1) / mw, mw * t.block_y, 0, s>>>(C, t, mw, ws, mean, var, running_mean, running_var, mom, bessel);
-  }
+  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
+  k_bn2d_stats<kBnStatsUnroll><<<rg.grid, rg.block, 0, s>>>(static_cast<const uint16_t*>(x), M, C, t, rg.vw, mean, var, running_mean,
+                                                           running_var, mom, bessel, ws);
+  if (t.grid_y > 1)
+    k_bn2d_stats_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, mean, var, running_mean, running_var, mom, bessel);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm statistics kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
@@ -1795,15 +1793,11 @@ int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t cha
   DeviceGuard g(device);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   float* ws = static_cast<float*>(workspace);
-  const int vw = bn::reduce_vecs(t, C);
-  k_bn2d_bwd_reduce<kBnReduceUnroll><<<dim3((C / 8 + vw - 1) / vw, t.grid_y), vw * t.block_y * bn::kAtenLoads, 0, s>>>(
-      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), M, C, t, vw, mean, invstd, sum_dy, sum_dy_xmu, grad_weight,
-      grad_bias, ws);
-  if (t.grid_y > 1) {
-    const int mw = bn::merge_vecs(t, C);
-    k_bn2d_bwd_reduce_merge<<<(C / 8 + mw - 1) / mw, mw * t.block_y, 0, s>>>(C, t, mw, ws, invstd, sum_dy, sum_dy_xmu, grad_weight,
-                                                                             grad_bias);
-  }
+  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
+  k_bn2d_bwd_reduce<kBnReduceUnroll><<<rg.grid, rg.block, 0, s>>>(static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), M, C, t,
+                                                                 rg.vw, mean, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias, ws);
+  if (t.grid_y > 1)
+    k_bn2d_bwd_reduce_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward reduce kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;

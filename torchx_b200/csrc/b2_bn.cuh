@@ -133,17 +133,29 @@ inline Tree tree(int M, int C) {
 }
 
 // Our CTA: `vw` vecs x block_y x the 4 slots, one chain of 8 channels per thread (vec fastest, so a warp reads whole
-// rows); one CTA row per ATen CTA row (blockIdx.y = by).  block_y <= 512 / 8, so a CTA has at most 256 threads.
-inline int reduce_vecs(const Tree& t, int C) {
-  const int per = t.block_y * kAtenLoads;
-  const int vw = kBnThreads / per > 1 ? kBnThreads / per : 1;
-  return vw < C / 8 ? vw : C / 8;
+// rows); one CTA row per ATen CTA row (blockIdx.y = by).  block_y <= 512 / 8, so a CTA has at most 256 threads.  The
+// grid_y merge: `mw` vecs x block_y threads per CTA.  reduce_rows and reduce_partials decode these from threadIdx.x.
+struct ReduceGrid {
+  int vw, block;
+  dim3 grid;
+  int mw, merge_block, merge_grid;
+};
+
+inline ReduceGrid reduce_grid(const Tree& t, int C) {
+  const auto vecs = [C](int per) {  // vecs of `per` threads each in one CTA
+    const int w = kBnThreads / per > 1 ? kBnThreads / per : 1;
+    return w < C / 8 ? w : C / 8;
+  };
+  ReduceGrid g;
+  g.vw = vecs(t.block_y * kAtenLoads);
+  g.block = g.vw * t.block_y * kAtenLoads;
+  g.grid = dim3((C / 8 + g.vw - 1) / g.vw, t.grid_y);
+  g.mw = vecs(t.block_y);
+  g.merge_block = g.mw * t.block_y;
+  g.merge_grid = (C / 8 + g.mw - 1) / g.mw;
+  return g;
 }
-// The grid_y merge: `vw` vecs x block_y threads per CTA.
-inline int merge_vecs(const Tree& t, int C) {
-  const int vw = kBnThreads / t.block_y > 1 ? kBnThreads / t.block_y : 1;
-  return vw < C / 8 ? vw : C / 8;
-}
+
 // Partials of the grid_y merge, float [by][C] mean (sum_dy) and m2n (sum_dy_xmu) and, for the statistics, int [by][C/8]
 // counts: ATen's staging, 3 words per (channel, by) there.
 inline size_t workspace_bytes(const Tree& t, int C) {
@@ -152,6 +164,7 @@ inline size_t workspace_bytes(const Tree& t, int C) {
 
 // Welford state of one chain over 8 channels (the count is the same for all 8: rows are valid for a whole vec or not at all).
 struct Welford {
+  static constexpr int kIn = 1;  // inputs: x
   int n;
   float mean[8], m2n[8];
 };
@@ -175,12 +188,70 @@ __device__ __forceinline__ void welford_merge(Welford& a, int cn, const float (&
   a.n = tot;
 }
 
+// The backward reduce's state of one chain over 8 channels: sum_dy and sum_dy_xmu.  The member order is deliberate: it
+// decides how ptxas assigns registers in both reduce kernels.
+struct Sums {
+  static constexpr int kIn = 2;  // inputs: dy, x
+  float xmu[8], dy[8];
+};
+
 // Shared-memory slots of a CTA's states: [8][256] means and m2ns (sum_dy / sum_dy_xmu), [256] counts.
 struct Smem {
   float a[8][kBnThreads];
   float b[8][kBnThreads];
   int n[kBnThreads];
 };
+
+// ---- what the reduction skeletons do with each state ---------------------------------------------------------------------
+// zero: the state a chain starts from.  begin: the chain's per-channel constants m (the backward's mean), loaded only by
+// threads with a vec.  update: one row of the inputs; `in` = the row is below M.
+
+__device__ __forceinline__ void zero(Welford& w) {
+  w.n = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) w.mean[k] = w.m2n[k] = 0.0f;
+}
+
+__device__ __forceinline__ void zero(Sums& s) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) s.dy[k] = s.xmu[k] = 0.0f;
+}
+
+__device__ __forceinline__ void begin(const Welford&, float (&)[8], const float*, unsigned long long) {}
+
+__device__ __forceinline__ void begin(const Sums&, float (&m)[8], const float* mean, unsigned long long col) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) m[k] = mean[col + k];
+}
+
+// ATen's Welford update in ATen's contraction (delta0 = x - mean; mean = FFMA delta0, 1/count, mean; delta1 = x - mean;
+// m2n = FFMA delta0*delta1, is_valid, m2n), one IEEE reciprocal of the count per row for all 8 channels.  A slot past M
+// still runs the update with x = 0, 1/count = 0, is_valid = 0, as ATen's does: that is not a no-op once the mean is inf
+// or NaN.
+__device__ __forceinline__ void update(Welford& w, const float (&)[8], bool in, const float (&f)[1][8]) {
+  float inv = 0.0f, valid = 0.0f;
+  if (in) {
+    ++w.n;
+    inv = __frcp_rn(__int2float_rn(w.n));
+    valid = 1.0f;
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float d0 = __fsub_rn(f[0][k], w.mean[k]);
+    w.mean[k] = __fmaf_rn(d0, inv, w.mean[k]);
+    const float d1 = __fsub_rn(f[0][k], w.mean[k]);
+    w.m2n[k] = __fmaf_rn(__fmul_rn(d0, d1), valid, w.m2n[k]);
+  }
+}
+
+// sum_dy += dy (FADD), sum_dy_xmu = FFMA (x - mean), dy, sum_dy_xmu; a slot past M adds dy = 0 and 0 * (0 - mean).
+__device__ __forceinline__ void update(Sums& s, const float (&m)[8], bool, const float (&f)[2][8]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    s.dy[k] = __fadd_rn(s.dy[k], f[0][k]);
+    s.xmu[k] = __fmaf_rn(__fsub_rn(f[1][k], m[k]), f[0][k], s.xmu[k]);
+  }
+}
 
 __device__ __forceinline__ void put(Smem& s, int slot, const Welford& w) {
 #pragma unroll
@@ -202,29 +273,67 @@ __device__ __forceinline__ void merge_from(Welford& w, const Smem& s, int slot) 
   welford_merge<kSlots>(w, s.n[slot], mn, m2);
 }
 
-__device__ __forceinline__ void put(Smem& s, int slot, const float (&a)[8], const float (&b)[8]) {
+__device__ __forceinline__ void put(Smem& s, int slot, const Sums& w) {
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    s.a[k][slot] = a[k];
-    s.b[k][slot] = b[k];
+    s.a[k][slot] = w.dy[k];
+    s.b[k][slot] = w.xmu[k];
   }
 }
 
-__device__ __forceinline__ void add_from(float (&a)[8], float (&b)[8], const Smem& s, int slot) {
+// Every merge of the sums is one FADD, the slots' as the tree's.
+template <bool kSlots>
+__device__ __forceinline__ void merge_from(Sums& w, const Smem& s, int slot) {
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    a[k] = __fadd_rn(a[k], s.a[k][slot]);
-    b[k] = __fadd_rn(b[k], s.b[k][slot]);
+    w.dy[k] = __fadd_rn(w.dy[k], s.a[k][slot]);
+    w.xmu[k] = __fadd_rn(w.xmu[k], s.b[k][slot]);
+  }
+}
+
+// CTA row blockIdx.y's partial into the workspace.
+__device__ __forceinline__ void store_partial(float* ws, int grid_y, int C, unsigned long long col, int vec, const Welford& w) {
+  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    ws[base + k] = w.mean[k];
+    ws[static_cast<size_t>(grid_y) * C + base + k] = w.m2n[k];
+  }
+  reinterpret_cast<int*>(ws + 2 * static_cast<size_t>(grid_y) * C)[static_cast<size_t>(blockIdx.y) * (C / 8) + vec] = w.n;
+}
+
+__device__ __forceinline__ void store_partial(float* ws, int grid_y, int C, unsigned long long col, int, const Sums& s) {
+  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    ws[base + k] = s.dy[k];
+    ws[static_cast<size_t>(grid_y) * C + base + k] = s.xmu[k];
+  }
+}
+
+// Merges CTA row y's partial, whose two float halves the skeleton has read into a and b (cnt: the statistics' counts).
+__device__ __forceinline__ void fold_partial(Welford& w, const float (&a)[8], const float (&b)[8], const int* cnt, int C, int vec, int y) {
+  welford_merge<false>(w, cnt[static_cast<size_t>(y) * (C / 8) + vec], a, b);
+}
+
+__device__ __forceinline__ void fold_partial(Sums& s, const float (&a)[8], const float (&b)[8], const int*, int, int, int) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    s.dy[k] = __fadd_rn(s.dy[k], a[k]);
+    s.xmu[k] = __fadd_rn(s.xmu[k], b[k]);
   }
 }
 
 // ATen's welford_merge_block_vertical / merge_block_vertical_backward over ty (slot = v + vw * ty): ty < off takes ty + off
 // for off = block_y/2 .. 1.  Every thread of the CTA calls it; `live` threads hold a state.
-template <class Merge>
-__device__ __forceinline__ void vertical(int v, int vw, int ty, int block_y, bool live, Merge&& merge) {
+template <class S>
+__device__ __forceinline__ void vertical(Smem& sm, S& s, int v, int vw, int ty, int block_y, bool live) {
   for (int off = block_y / 2; off > 0; off >>= 1) {
     __syncthreads();
-    if (live && ty < off) merge(v + vw * (ty + off), v + vw * ty);
+    if (live && ty < off) {
+      merge_from<false>(s, sm, v + vw * (ty + off));
+      put(sm, v + vw * ty, s);
+    }
   }
 }
 
@@ -248,16 +357,136 @@ __device__ __forceinline__ void stats_out(const Welford& w, unsigned long long c
 }
 
 // The end of ATen's backward reduce: grad_weight = sum_dy_xmu * invstd (FMUL), grad_bias = sum_dy.
-__device__ __forceinline__ void reduce_out(const float (&sdy)[8], const float (&sxmu)[8], unsigned long long col, const float* __restrict__ invstd,
-                                           float* __restrict__ sum_dy, float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight,
-                                           float* __restrict__ grad_bias) {
+__device__ __forceinline__ void reduce_out(const Sums& s, unsigned long long col, const float* __restrict__ invstd, float* __restrict__ sum_dy,
+                                           float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight, float* __restrict__ grad_bias) {
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    sum_dy[col + k] = sdy[k];
-    sum_dy_xmu[col + k] = sxmu[k];
-    grad_weight[col + k] = __fmul_rn(sxmu[k], invstd[col + k]);
-    grad_bias[col + k] = sdy[k];
+    sum_dy[col + k] = s.dy[k];
+    sum_dy_xmu[col + k] = s.xmu[k];
+    grad_weight[col + k] = __fmul_rn(s.xmu[k], invstd[col + k]);
+    grad_bias[col + k] = s.dy[k];
   }
+}
+
+// ---- the skeletons ------------------------------------------------------------------------------------------------------
+// The elementwise passes: each CTA row walks its row blocks of p.rows * U rows, last one first, with U rows' loads of
+// every input issued before the first is used.  f(in, out) maps one row's 8 channels of the kIn inputs to the output's.
+template <int U, int kIn, class F>
+__device__ __forceinline__ void elemt_rows(const Lane& l, const Plan& p, unsigned long long M, unsigned long long C,
+                                           const uint16_t* __restrict__ in0, const uint16_t* __restrict__ in1, uint16_t* __restrict__ out,
+                                           F&& f) {
+  const unsigned long long step = static_cast<unsigned long long>(p.rows) * U;
+  const unsigned long long stride = step * p.gy;
+  const unsigned long long first = blockIdx.y * step;
+  if (first >= M) return;
+  for (long long base = static_cast<long long>(first + (M - 1 - first) / stride * stride); base >= 0; base -= stride) {
+    uint4 q[U][kIn];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const unsigned long long row = base + u * p.rows + l.r;
+      q[u][0] = row < M ? ld_vec(in0 + row * C + l.col) : make_uint4(0, 0, 0, 0);
+      if constexpr (kIn == 2) q[u][1] = row < M ? ld_vec(in1 + row * C + l.col) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const unsigned long long row = base + u * p.rows + l.r;
+      if (row < M) {
+        float fi[kIn][8], fo[8];
+#pragma unroll
+        for (int i = 0; i < kIn; ++i) unpack(q[u][i], fi[i]);
+        f(fi, fo);
+        *reinterpret_cast<uint4*>(out + row * C + l.col) = pack(fo);
+      }
+    }
+  }
+}
+
+// The reductions: thread (vec, ty, j) of ATen CTA row by = blockIdx.y runs its chain of state S over the S::kIn inputs
+// (in0, in1), with U rows' loads issued before the first is used; then the slot merge and the vertical merge through
+// shared memory.  With grid_y == 1 the CTA hands each vec's state to out(state, col), otherwise it writes its partial,
+// which reduce_partials folds.  `mean` feeds begin (the backward's; null for the statistics).
+template <int U, class S, class Out>
+__device__ __forceinline__ void reduce_rows(const uint16_t* in0, const uint16_t* in1, int M, int C, const Tree& t, int vw, const float* mean,
+                                            float* ws, Out&& out) {
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  S s;
+  zero(s);
+  float m[8];
+  if (on) {
+    begin(s, m, mean, col);
+    const int stride = kAtenLoads * t.seq;
+    int row = blockIdx.y * t.block_y + ty + j * t.seq;
+    for (int i = 0; i < t.loops; i += U) {
+      uint4 q[U][S::kIn];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int r = row + u * stride;
+        const bool ld = i + u < t.loops && r < M;
+        q[u][0] = ld ? ld_vec(in0 + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+        if constexpr (S::kIn == 2) q[u][1] = ld ? ld_vec(in1 + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (i + u < t.loops) {
+          float f[S::kIn][8];
+#pragma unroll
+          for (int n = 0; n < S::kIn; ++n) unpack(q[u][n], f[n]);
+          update(s, m, row + u * stride < M, f);
+        }
+      }
+      row += U * stride;
+    }
+  }
+  put(sm, v + vw * (ty + t.block_y * j), s);
+  __syncthreads();
+  const bool lead = on && j == 0;
+  if (lead) {
+#pragma unroll
+    for (int jj = 1; jj < kAtenLoads; ++jj) merge_from<true>(s, sm, v + vw * (ty + t.block_y * jj));
+    put(sm, v + vw * ty, s);
+  }
+  vertical(sm, s, v, vw, ty, t.block_y, lead);
+  if (!lead || ty != 0) return;
+  if (t.grid_y == 1) {
+    out(s, col);
+    return;
+  }
+  store_partial(ws, t.grid_y, C, col, vec, s);
+}
+
+// ATen's last block: thread ty folds partials y = ty, ty + block_y, ... into a zero state, then the vertical merge, and
+// ty = 0 hands each vec's state to out(state, col).
+template <class S, class Out>
+__device__ __forceinline__ void reduce_partials(int C, const Tree& t, int vw, const float* ws, Out&& out) {
+  __shared__ Smem sm;
+  const int tid = threadIdx.x;
+  const int v = tid % vw, ty = tid / vw;
+  const int vec = blockIdx.x * vw + v;
+  const bool on = vec < C / 8;
+  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
+  const int* cnt = reinterpret_cast<const int*>(ws + 2 * static_cast<size_t>(t.grid_y) * C);
+  S s;
+  zero(s);
+  if (on) {
+    for (int y = ty; y < t.grid_y; y += t.block_y) {
+      const size_t base = static_cast<size_t>(y) * C + col;
+      float a[8], b[8];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        a[k] = ws[base + k];
+        b[k] = ws[static_cast<size_t>(t.grid_y) * C + base + k];
+      }
+      fold_partial(s, a, b, cnt, C, vec, y);
+    }
+    put(sm, v + vw * ty, s);
+  }
+  vertical(sm, s, v, vw, ty, t.block_y, on);
+  if (on && ty == 0) out(s, col);
 }
 
 }  // namespace bn
@@ -285,30 +514,10 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
 #pragma unroll
     for (int k = 0; k < 8; ++k) save_invstd[l.col + k] = is[k];
   }
-  const unsigned long long step = static_cast<unsigned long long>(p.rows) * U;
-  const unsigned long long stride = step * p.gy;
-  const unsigned long long first = blockIdx.y * step;
-  if (first >= M) return;
-  // last row block first
-  for (long long base = static_cast<long long>(first + (M - 1 - first) / stride * stride); base >= 0; base -= stride) {
-    uint4 q[U];
+  elemt_rows<U, 1>(l, p, M, C, x, nullptr, y, [&](const float (&f)[1][8], float (&o)[8]) {
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const unsigned long long row = base + u * p.rows + l.r;
-      q[u] = row < M ? ld_vec(x + row * C + l.col) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const unsigned long long row = base + u * p.rows + l.r;
-      if (row < M) {
-        float f[8];
-        unpack(q[u], f);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) f[k] = w[k] * (f[k] - m[k]) * is[k] + b[k];
-        *reinterpret_cast<uint4*>(y + row * C + l.col) = pack(f);
-      }
-    }
-  }
+    for (int k = 0; k < 8; ++k) o[k] = w[k] * (f[0][k] - m[k]) * is[k] + b[k];
+  });
 }
 
 // ---- backward elementwise ------------------------------------------------------------------------------------------------
@@ -332,154 +541,37 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
     f2[k] = weight[c] * is;
     f1[k] = is * is * sum_dy_xmu[c] * norm_fct;
   }
-  const unsigned long long step = static_cast<unsigned long long>(p.rows) * U;
-  const unsigned long long stride = step * p.gy;
-  const unsigned long long first = blockIdx.y * step;
-  if (first >= M) return;
-  for (long long base = static_cast<long long>(first + (M - 1 - first) / stride * stride); base >= 0; base -= stride) {
-    uint4 qd[U], qx[U];
+  elemt_rows<U, 2>(l, p, M, C, dy, x, dx, [&](const float (&f)[2][8], float (&o)[8]) {
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const unsigned long long row = base + u * p.rows + l.r;
-      qd[u] = row < M ? ld_vec(dy + row * C + l.col) : make_uint4(0, 0, 0, 0);
-      qx[u] = row < M ? ld_vec(x + row * C + l.col) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const unsigned long long row = base + u * p.rows + l.r;
-      if (row < M) {
-        float fd[8], fx[8];
-        unpack(qd[u], fd);
-        unpack(qx[u], fx);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) fd[k] = (fd[k] - mdy[k] - (fx[k] - m[k]) * f1[k]) * f2[k];
-        *reinterpret_cast<uint4*>(dx + row * C + l.col) = pack(fd);
-      }
-    }
-  }
+    for (int k = 0; k < 8; ++k) o[k] = (f[0][k] - mdy[k] - (f[1][k] - m[k]) * f1[k]) * f2[k];
+  });
 }
 
 // ---- forward statistics -------------------------------------------------------------------------------------------------
-// One thread per (vec, ty, j) of ATen CTA row by = blockIdx.y: the chain's Welford update per row in ATen's contraction
-// (delta0 = x - mean; mean = FFMA delta0, 1/count, mean; delta1 = x - mean; m2n = FFMA delta0*delta1, is_valid, m2n), one
-// IEEE reciprocal of the count per row for all 8 channels.  A slot past M still runs the update with x = 0, 1/count = 0,
-// is_valid = 0, as ATen's does: that is not a no-op once the mean is inf or NaN.  U rows' loads are issued before the
-// first is used.  Then the slot merge and the vertical merge through shared memory; with grid_y == 1 the CTA writes the
-// outputs, otherwise its partial, which k_bn2d_stats_merge folds in ATen's last-block order.
+// ATen's Welford chains; the merge kernel folds the CTA rows' partials in ATen's last-block order and, like the main
+// kernel with grid_y == 1, writes mean, var = m2n / M and the running statistics.
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads)
     k_bn2d_stats(const uint16_t* __restrict__ x, int M, int C, bn::Tree t, int vw, float* __restrict__ mean, float* __restrict__ var,
                  float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel, float* __restrict__ ws) {
   using namespace bn;
-  __shared__ Smem sm;
-  const int tid = threadIdx.x;
-  const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
-  const int vec = blockIdx.x * vw + v;
-  const bool on = vec < C / 8;
-  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
-  Welford w;
-  w.n = 0;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) w.mean[k] = w.m2n[k] = 0.0f;
-  if (on) {
-    const int stride = kAtenLoads * t.seq;
-    int row = blockIdx.y * t.block_y + ty + j * t.seq;
-    for (int i = 0; i < t.loops; i += U) {
-      uint4 q[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int r = row + u * stride;
-        q[u] = i + u < t.loops && r < M ? ld_vec(x + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if (i + u < t.loops) {
-          float inv = 0.0f, valid = 0.0f;
-          if (row + u * stride < M) {
-            ++w.n;
-            inv = __frcp_rn(__int2float_rn(w.n));
-            valid = 1.0f;
-          }
-          float f[8];
-          unpack(q[u], f);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const float d0 = __fsub_rn(f[k], w.mean[k]);
-            w.mean[k] = __fmaf_rn(d0, inv, w.mean[k]);
-            const float d1 = __fsub_rn(f[k], w.mean[k]);
-            w.m2n[k] = __fmaf_rn(__fmul_rn(d0, d1), valid, w.m2n[k]);
-          }
-        }
-      }
-      row += U * stride;
-    }
-  }
-  put(sm, v + vw * (ty + t.block_y * j), w);
-  __syncthreads();
-  const bool lead = on && j == 0;
-  if (lead) {
-#pragma unroll
-    for (int jj = 1; jj < kAtenLoads; ++jj) merge_from<true>(w, sm, v + vw * (ty + t.block_y * jj));
-    put(sm, v + vw * ty, w);
-  }
-  vertical(v, vw, ty, t.block_y, lead, [&](int src, int dst) {
-    merge_from<false>(w, sm, src);
-    put(sm, dst, w);
-  });
-  if (!lead || ty != 0) return;
-  if (t.grid_y == 1) {
+  reduce_rows<U, Welford>(x, nullptr, M, C, t, vw, nullptr, ws, [&](const Welford& w, unsigned long long col) {
     stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
-    return;
-  }
-  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    ws[base + k] = w.mean[k];
-    ws[static_cast<size_t>(t.grid_y) * C + base + k] = w.m2n[k];
-  }
-  reinterpret_cast<int*>(ws + 2 * static_cast<size_t>(t.grid_y) * C)[static_cast<size_t>(blockIdx.y) * (C / 8) + vec] = w.n;
+  });
 }
 
-// ATen's last block: thread ty merges partials y = ty, ty + block_y, ... into a zero state, then the vertical merge.
 __global__ void __launch_bounds__(bn::kBnThreads)
     k_bn2d_stats_merge(int C, bn::Tree t, int vw, const float* __restrict__ ws, float* __restrict__ mean, float* __restrict__ var,
                        float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel) {
   using namespace bn;
-  __shared__ Smem sm;
-  const int tid = threadIdx.x;
-  const int v = tid % vw, ty = tid / vw;
-  const int vec = blockIdx.x * vw + v;
-  const bool on = vec < C / 8;
-  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
-  const int* cnt = reinterpret_cast<const int*>(ws + 2 * static_cast<size_t>(t.grid_y) * C);
-  Welford w;
-  w.n = 0;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) w.mean[k] = w.m2n[k] = 0.0f;
-  if (on) {
-    for (int y = ty; y < t.grid_y; y += t.block_y) {
-      const size_t base = static_cast<size_t>(y) * C + col;
-      float mn[8], m2[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        mn[k] = ws[base + k];
-        m2[k] = ws[static_cast<size_t>(t.grid_y) * C + base + k];
-      }
-      welford_merge<false>(w, cnt[static_cast<size_t>(y) * (C / 8) + vec], mn, m2);
-    }
-    put(sm, v + vw * ty, w);
-  }
-  vertical(v, vw, ty, t.block_y, on, [&](int src, int dst) {
-    merge_from<false>(w, sm, src);
-    put(sm, dst, w);
+  reduce_partials<Welford>(C, t, vw, ws, [&](const Welford& w, unsigned long long col) {
+    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
   });
-  if (on && ty == 0) stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
 }
 
 // ---- backward reduce ----------------------------------------------------------------------------------------------------
-// The same chains with plain sums: sum_dy += dy (FADD), sum_dy_xmu = FFMA (x - mean), dy, sum_dy_xmu; a slot past M adds
-// dy = 0 and 0 * (0 - mean).  ATen's kernel returns early from threads with c_offset >= C or m_offset >= M: the first only
-// ever holds channels no valid thread reads (the vertical merge pairs threads of one threadIdx.x), and m_offset =
+// The same tree with plain sums.  ATen's kernel returns early from threads with c_offset >= C or m_offset >= M: the first
+// only ever holds channels no valid thread reads (the vertical merge pairs threads of one threadIdx.x), and m_offset =
 // by*block_y + ty < block_y*grid_y <= M for every geometry flexible_launch_configs makes, so no valid channel is affected.
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads)
@@ -488,100 +580,17 @@ __global__ void __launch_bounds__(bn::kBnThreads)
                       float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight, float* __restrict__ grad_bias,
                       float* __restrict__ ws) {
   using namespace bn;
-  __shared__ Smem sm;
-  const int tid = threadIdx.x;
-  const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
-  const int vec = blockIdx.x * vw + v;
-  const bool on = vec < C / 8;
-  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
-  float sdy[8], sxmu[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) sdy[k] = sxmu[k] = 0.0f;
-  if (on) {
-    float m[8];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) m[k] = mean[col + k];
-    const int stride = kAtenLoads * t.seq;
-    int row = blockIdx.y * t.block_y + ty + j * t.seq;
-    for (int i = 0; i < t.loops; i += U) {
-      uint4 qd[U], qx[U];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int r = row + u * stride;
-        const bool ld = i + u < t.loops && r < M;
-        qd[u] = ld ? ld_vec(dy + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
-        qx[u] = ld ? ld_vec(x + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if (i + u < t.loops) {
-          float fd[8], fx[8];
-          unpack(qd[u], fd);
-          unpack(qx[u], fx);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            sdy[k] = __fadd_rn(sdy[k], fd[k]);
-            sxmu[k] = __fmaf_rn(__fsub_rn(fx[k], m[k]), fd[k], sxmu[k]);
-          }
-        }
-      }
-      row += U * stride;
-    }
-  }
-  put(sm, v + vw * (ty + t.block_y * j), sdy, sxmu);
-  __syncthreads();
-  const bool lead = on && j == 0;
-  if (lead) {
-#pragma unroll
-    for (int jj = 1; jj < kAtenLoads; ++jj) add_from(sdy, sxmu, sm, v + vw * (ty + t.block_y * jj));
-    put(sm, v + vw * ty, sdy, sxmu);
-  }
-  vertical(v, vw, ty, t.block_y, lead, [&](int src, int dst) {
-    add_from(sdy, sxmu, sm, src);
-    put(sm, dst, sdy, sxmu);
+  reduce_rows<U, Sums>(dy, x, M, C, t, vw, mean, ws, [&](const Sums& s, unsigned long long col) {
+    reduce_out(s, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
   });
-  if (!lead || ty != 0) return;
-  if (t.grid_y == 1) {
-    reduce_out(sdy, sxmu, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
-    return;
-  }
-  const size_t base = static_cast<size_t>(blockIdx.y) * C + col;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    ws[base + k] = sdy[k];
-    ws[static_cast<size_t>(t.grid_y) * C + base + k] = sxmu[k];
-  }
 }
 
-// ATen's last block for the sums: from 0, add partials y = ty, ty + block_y, ..., then the vertical merge.
 __global__ void __launch_bounds__(bn::kBnThreads)
     k_bn2d_bwd_reduce_merge(int C, bn::Tree t, int vw, const float* __restrict__ ws, const float* __restrict__ invstd,
                             float* __restrict__ sum_dy, float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight,
                             float* __restrict__ grad_bias) {
   using namespace bn;
-  __shared__ Smem sm;
-  const int tid = threadIdx.x;
-  const int v = tid % vw, ty = tid / vw;
-  const int vec = blockIdx.x * vw + v;
-  const bool on = vec < C / 8;
-  const unsigned long long col = static_cast<unsigned long long>(vec) * 8;
-  float sdy[8], sxmu[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) sdy[k] = sxmu[k] = 0.0f;
-  if (on) {
-    for (int y = ty; y < t.grid_y; y += t.block_y) {
-      const size_t base = static_cast<size_t>(y) * C + col;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        sdy[k] = __fadd_rn(sdy[k], ws[base + k]);
-        sxmu[k] = __fadd_rn(sxmu[k], ws[static_cast<size_t>(t.grid_y) * C + base + k]);
-      }
-    }
-    put(sm, v + vw * ty, sdy, sxmu);
-  }
-  vertical(v, vw, ty, t.block_y, on, [&](int src, int dst) {
-    add_from(sdy, sxmu, sm, src);
-    put(sm, dst, sdy, sxmu);
+  reduce_partials<Sums>(C, t, vw, ws, [&](const Sums& s, unsigned long long col) {
+    reduce_out(s, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
   });
-  if (on && ty == 0) reduce_out(sdy, sxmu, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
 }
