@@ -163,8 +163,16 @@ int b2_auto_algo(int world, int mode, size_t n_elems, int has_multicast);
  *   "ll_max_bytes"       ... up to (excluding) this many                (env B2_LL_MAX_BYTES)
  *   "pipe_chunk_bytes"   target wire bytes per pipeline chunk           (env B2_PIPE_CHUNK_KB, in KiB)
  *   "max_ctas"           same as b2_comm_set_max_ctas
+ * And one test and diagnostic knob:
+ *   "op_count"           sets the device op counter (see b2_comm_op_count) to `value`, so that a test can run collectives
+ *                        where a long-lived communicator's counter would be.  Only while the communicator is idle, with
+ *                        the same value on every rank; synchronises the device, then copies the value.
  */
 int b2_comm_set_param(b2_comm_t* comm, const char* name, long long value);
+
+/* The device op counter: the number of collectives this communicator has completed, plus any "op_count" it was given.
+ * Point-to-point does not count.  A synchronous copy; 0 with b2_last_error() set if `comm` is NULL or the copy fails. */
+uint64_t b2_comm_op_count(const b2_comm_t* comm);
 
 /*
  * Non-blocking health check: B2_OK, B2_ETIMEOUT if any kernel of this communicator gave up

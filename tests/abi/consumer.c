@@ -21,6 +21,8 @@ typedef const char* (*last_error_fn)(void);
 typedef int (*allreduce_fn)(b2_comm_t*, void*, size_t, int, float, int, void*);
 typedef int (*destroy_fn)(b2_comm_t*);
 typedef int (*auto_algo_fn)(int, int, size_t, int);
+typedef int (*set_param_fn)(b2_comm_t*, const char*, long long);
+typedef uint64_t (*op_count_fn)(const b2_comm_t*);
 
 int main(int argc, char** argv) {
   static const char* const symbols[] = {B2_CONSUMER_SYMBOLS};
@@ -31,6 +33,8 @@ int main(int argc, char** argv) {
   allreduce_fn allreduce;
   destroy_fn destroy;
   auto_algo_fn auto_algo;
+  set_param_fn set_param;
+  op_count_fn op_count;
   b2_segment_t seg;
 
   CHECK(argc == 2);
@@ -57,6 +61,10 @@ int main(int argc, char** argv) {
   CHECK(auto_algo(8, B2_F32_WIRE_BF16, (size_t)1 << 28, 1) == B2_ALGO_NVLS); /* 1 GiB of fp32 at W=8 with multicast */
   CHECK(auto_algo(8, B2_F32_WIRE_BF16, (size_t)1 << 28, 0) == B2_ALGO_TWOSHOT);
   CHECK(auto_algo(8, B2_F32_WIRE_BF16, 1024, 0) == B2_ALGO_ONESHOT);
+  *(void**)(&set_param) = dlsym(lib, "b2_comm_set_param");
+  *(void**)(&op_count) = dlsym(lib, "b2_comm_op_count");
+  CHECK(set_param(NULL, "op_count", 1) == B2_EINVAL);
+  CHECK(op_count(NULL) == 0 && strstr(last_error(), "null communicator") != NULL);
   /* plain-data layout of the one struct that crosses the boundary */
   memset(&seg, 0, sizeof seg);
   CHECK(sizeof seg == sizeof(void*) + 2 * sizeof(uint64_t));

@@ -82,3 +82,4 @@ def test_argument_validation_without_a_gpu():
     assert L.b2_allreduce_gather(None, None, 0, None, 0, 0, 1.0, 0, None) == N.B2_OK  # n_elems == 0: a no-op, table unread
     assert L.b2_comm_caps(None) == N.B2_EINVAL and L.b2_comm_last_algo(None) == N.B2_EINVAL
     assert L.b2_comm_set_param(None, b"max_ctas", 1) == N.B2_EINVAL
+    assert L.b2_comm_op_count(None) == 0 and b"b2_comm_op_count: null communicator" in L.b2_last_error()

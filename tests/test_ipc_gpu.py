@@ -16,13 +16,13 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run_world(world, devices, tmp_path, n=100003):
+def _run_world(world, devices, tmp_path, n=100003, op_count=0):
     shm = f"/b2_test_{uuid.uuid4().hex[:12]}"
     procs = []
     for r in range(world):
         out = tmp_path / f"r{r}.npz"
         cmd = [sys.executable, os.path.join(ROOT, "tests", "workers", "ipc_worker.py"), "--rank", str(r), "--world",
-               str(world), "--device", str(devices[r]), "--shm", shm, "--n", str(n), "--out", str(out)]
+               str(world), "--device", str(devices[r]), "--shm", shm, "--n", str(n), "--out", str(out), "--op-count", str(op_count)]
         procs.append(subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
     outs = []
     try:
@@ -42,6 +42,7 @@ def _run_world(world, devices, tmp_path, n=100003):
             xs = make_inputs(world, n, 10 + k, "special")
             assert_bits_equal(got[f"ar{k}"], oracle.allreduce(mode, xs, 1.0 / world), f"rank {r} op {k}")
         assert np.all(got["bcast"] == float(world)), r
+        assert got["counted"].all(), f"rank {r}: the op counter did not advance by one per collective from {op_count}"
         assert_bits_equal(got["ll"], oracle.allreduce(oracle.B2O_F32_WIRE_BF16, make_inputs(world, n, 30, "special"), 1.0 / world), f"rank {r} LL two-shot")
         if "nvls" in got.files:  # the box exposes NVSwitch multicast: the worker also ran the NVLS algorithm
             assert_nvls_result(got["nvls"], make_inputs(world, n, 20, "randn"), 1.0 / world, oracle.B2O_F32_WIRE_BF16, f"nvls rank {r}")
@@ -50,6 +51,12 @@ def _run_world(world, devices, tmp_path, n=100003):
 
 def test_two_processes_share_one_device(tmp_path):
     _run_world(2, [0, 0], tmp_path, n=20011)
+
+
+def test_two_processes_share_one_device_from_op_count_2_29(tmp_path):
+    """Both ranks start their counter at 2^29, where a 32-bit flag compare would take a never-written slot for a current
+    one (tests/test_op_count_gpu.py)."""
+    _run_world(2, [0, 0], tmp_path, n=20011, op_count=1 << 29)
 
 
 def test_two_processes_share_one_device_cuda_ipc_backend(tmp_path, monkeypatch):

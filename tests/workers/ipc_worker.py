@@ -24,11 +24,14 @@ def main() -> None:
     ap.add_argument("--n", type=int, default=100003)
     ap.add_argument("--out", required=True)
     ap.add_argument("--max-ctas", type=int, default=8)
+    ap.add_argument("--op-count", type=int, default=0, help="the op counter every rank starts at")
     a = ap.parse_args()
 
     comm = Communicator.create(a.rank, a.world, a.device, a.shm, epoch=a.epoch, stage_mb=8, timeout_s=60)
     comm.set_timeout(30.0)
     comm.set_max_ctas(a.max_ctas)
+    if a.op_count:
+        comm.set_param("op_count", a.op_count)
     results = {}
     comm.set_param("pipe_chunk_bytes", 16 << 10)  # several pipeline chunks even at this message size
     for k, (algo, mode) in enumerate([("twoshot", "bf16"), ("oneshot", "bf16"), ("twoshot", "f32"), ("twoshot_pipe", "bf16")]):
@@ -54,6 +57,7 @@ def main() -> None:
     torch.cuda.synchronize()
     comm.check()
     results["bcast"] = b.cpu().numpy()
+    results["counted"] = np.array([comm.op_count - a.op_count == comm.launches])
     np.savez(a.out, **results)
     comm.close()
     print(f"rank {a.rank} ok", flush=True)

@@ -161,7 +161,7 @@ struct b2_comm {
   vmm::Mapping peers[B2_MAX_WORLD];  // VMM backend, multi-process: imported peer allocations
   vmm::Mapping mc;                   // VMM backend, multi-process: the multicast object
   LocalMc* local_mc = nullptr;       // VMM backend, in-process world
-  uint32_t* counters = nullptr;  // cudaMalloc'ed: opseq, done
+  uint32_t* counters = nullptr;  // cudaMalloc'ed, 256 B: opseq (u64, words 0-1), done (word 32)
   uint32_t* p2p_counters = nullptr;  // cudaMalloc'ed: chunks sent to [0, W) / received from [8, 8 + W) each rank; [32] done
   size_t p2p_off = 0;                // the point-to-point region of every arena (b2_p2p.cuh)
   unsigned long long* trace_dev = nullptr;  // cudaMalloc'ed on demand: kMaxCtas * 8 stamps
@@ -232,7 +232,7 @@ void layout(b2_comm* c, int world, size_t stage_bytes) {
   c->d.ll_off[0] = c->arena_bytes;
   c->d.ll_off[1] = c->arena_bytes + ll_bytes;
   c->arena_bytes += 2 * ll_bytes;
-  c->d.llflag_off = 32u << 10;  // inside the xbar flag region, past its kMaxCtas slots
+  c->d.llflag_off = kLLFlagOff;
   // point-to-point inboxes, flags and credits: after everything the collectives use, a function of the world size alone
   c->p2p_off = c->arena_bytes;
   c->arena_bytes += p2p_region_bytes(world);
@@ -262,7 +262,7 @@ int init_rank(b2_comm* c, int rank, int world, int device, size_t stage_bytes) {
   B2_CUDA(cudaSetDevice(device));
   B2_CUDA(cudaMalloc(&c->counters, 256));
   B2_CUDA(cudaMemset(c->counters, 0, 256));
-  c->d.opseq = c->counters;
+  c->d.opseq = reinterpret_cast<uint64_t*>(c->counters);
   c->d.done = c->counters + 32;  // a different 128 B line
   B2_CUDA(cudaMalloc(&c->p2p_counters, 256));
   B2_CUDA(cudaMemset(c->p2p_counters, 0, 256));
@@ -1041,8 +1041,29 @@ int b2_comm_set_param(b2_comm_t* c, const char* name, long long value) {
   else if (k == "ll_max_bytes") c->policy.ll_max = static_cast<size_t>(value);
   else if (k == "pipe_chunk_bytes") c->pipe_chunk_bytes = static_cast<size_t>(value);
   else if (k == "max_ctas") c->max_ctas = static_cast<int>(value);
+  else if (k == "op_count") {
+    const uint64_t v = static_cast<uint64_t>(value);
+    DeviceGuard g(c->device);
+    B2_CUDA(cudaDeviceSynchronize());  // the counter is only rewritten between collectives
+    B2_CUDA(cudaMemcpy(c->d.opseq, &v, sizeof(v), cudaMemcpyHostToDevice));
+  }
   else return fail(B2_EINVAL, "b2_comm_set_param: unknown parameter '%s'", name);
   return B2_OK;
+}
+
+uint64_t b2_comm_op_count(const b2_comm_t* c) {
+  if (!c) {
+    fail(B2_EINVAL, "b2_comm_op_count: null communicator");
+    return 0;
+  }
+  uint64_t v = 0;
+  DeviceGuard g(c->device);
+  const cudaError_t e = cudaMemcpy(&v, c->d.opseq, sizeof(v), cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) {
+    fail(B2_ECUDA, "b2_comm_op_count: %s", cudaGetErrorString(e));
+    return 0;
+  }
+  return v;
 }
 
 int b2_comm_status(const b2_comm_t* c) {

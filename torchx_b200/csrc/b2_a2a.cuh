@@ -40,7 +40,7 @@ constexpr size_t kA2aHeaderBytes = 16;  // at the start of every recv region; a 
 
 __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) {
   using namespace dev;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
   const unsigned long long first = static_cast<unsigned long long>(blockIdx.x) * kThreads + threadIdx.x;
@@ -92,5 +92,5 @@ __global__ void __launch_bounds__(kThreads, 1) k_alltoall(CommDev c, A2aArgs a) 
   } else if (blockIdx.x == 0 && threadIdx.x == 0 && ld_volatile_u32(c.status) == 0) {  // a timeout recorded first stays
     record_status(c.status, B2_EINVAL);
   }
-  op_end(c, seq0);
+  op_end(c);
 }

@@ -50,7 +50,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   const bool am = (reinterpret_cast<uintptr_t>(mean) & 15u) == 0;
   const bool ai = (reinterpret_cast<uintptr_t>(invstd) & 15u) == 0;
   const unsigned long long Cv = (C + 3) / 4;  // vecs of one statistic; the row is mean, invstd, then the count's vec
-  uint32_t seq0 = 0;
+  uint64_t seq0 = 0;
   const uint8_t* mine = nullptr;
   if (!solo) {
     seq0 = op_begin(c);
@@ -124,5 +124,5 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
   }
-  if (!solo) op_end(c, seq0);
+  if (!solo) op_end(c);
 }

@@ -16,11 +16,11 @@ namespace {
 
 constexpr int kThreads = 512;                // threads per CTA for every collective kernel
 constexpr int kMaxCtas = 264;                // 2 x 132 SMs (H100 SXM): upper bound on the grid of a collective
-constexpr int kFlagSlotBytes = 32;           // one 32 B sector of flags per slot (8 x u32, one per source rank)
+constexpr int kFlagSlotBytes = 64;           // one 64 B half-line of flags per slot (8 x u64, one per source rank)
 constexpr size_t kXbarFlagBytes = 64 << 10;  // region 0: one slot per CTA index (cta_xbar: one-shot, two-shot, broadcast, barrier)
 constexpr int kMaxChunks = 16;               // chunk slots per CTA index and kind in the pipeline flag region
 constexpr int kPipeKinds = 2;                // X1 ("inputs staged / scattered"), X2 ("slice reduced / multicast")
-constexpr size_t kPipeFlagBytes = 448 << 10;  // region 1: kMaxCtas x kPipeKinds x kMaxChunks slots; stages start 512 KiB in
+constexpr size_t kPipeFlagBytes = 960 << 10;  // region 1: kMaxCtas x kPipeKinds x kMaxChunks slots; stages start 1 MiB in
 constexpr size_t kFlagRegionBytes = kXbarFlagBytes + kPipeFlagBytes;
 constexpr size_t kDefaultStageBytes = 512ull << 20;  // x2 stages = 1 GiB of the 80 GB: a 1 GiB fp32 bucket is one launch
 // Peer waits are bounded so a dead peer can never wedge the GPU, but the bound has to be far above any legitimate
@@ -87,7 +87,9 @@ constexpr bool kF32Wire = ModeTraits<MODE>::kWire == WireFmt::kF32;  // 32-byte 
 template <int MODE>
 constexpr bool k16BitBucket = ModeTraits<MODE>::kElemBytes == 2;     // the bucket holds wire-format elements
 
-static_assert(kMaxCtas * kFlagSlotBytes <= (int)kXbarFlagBytes, "xbar flag region too small");
+constexpr size_t kLLFlagOff = 32 << 10;      // the LL flow-control words (8 x u64), inside region 0 past its slots
+static_assert((size_t)kMaxCtas * kFlagSlotBytes <= kLLFlagOff && kLLFlagOff + kFlagSlotBytes <= kXbarFlagBytes,
+              "xbar flag region too small");
 static_assert((size_t)kMaxCtas * kPipeKinds * kMaxChunks * kFlagSlotBytes <= kPipeFlagBytes, "pipeline flag region too small");
 
 // Device-visible description of one rank's view of the communicator; passed BY VALUE as a kernel
@@ -103,7 +105,7 @@ struct CommDev {
   uint8_t* mc;                      // multicast (NVLS) alias of the arena: a store to mc + off lands at arena + off on
                                     // EVERY rank, a multimem.ld_reduce from it returns the switch-side sum over all
                                     // ranks; nullptr when the fabric / driver does not expose multicast
-  uint32_t* opseq;                  // local: number of collectives completed on this communicator
+  uint64_t* opseq;                  // local: number of collectives completed on this communicator
   uint32_t* done;                   // local: CTAs of the running collective that reached the epilogue
   uint32_t* status;                 // host-mapped: 0 = healthy, else a B2_E* code (positive)
   unsigned long long timeout_ns;    // bound on any single peer wait
@@ -120,7 +122,7 @@ struct CommDev {
                                     // Always all-SENTINEL outside a running collective: a consumer recognises arrived data
                                     // word by word as "not the sentinel" (no flag, no fence, no barrier) and puts the
                                     // sentinel back after reading.
-  unsigned long long llflag_off;    // 8 x u32: llflag[r] = op counter of the latest LL collective rank r has STARTED
+  unsigned long long llflag_off;    // 8 x u64: llflag[r] = op counter of the latest LL collective rank r has STARTED
                                     // (flow control: nobody writes a parity's buffers before their owner has left the
                                     // collective that last used them)
   unsigned long long* trace;        // optional (b2_comm_trace): per-CTA globaltimer stamps of the LAST collective,
@@ -168,6 +170,19 @@ __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
 __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
   uint32_t v;
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_sys(uint64_t* p, uint64_t v) {
+  asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ uint64_t ld_acquire_sys(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint64_t ld_volatile_u64(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
   return v;
 }
 __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
@@ -658,13 +673,14 @@ __device__ __forceinline__ void record_status(uint32_t* status, int code) {
   __threadfence_system();
 }
 
-// Bounded wait until *flag >= seq (wrap-safe).  Polls with ld.acquire.sys itself rather than relaxed polling + one
-// fence.acq_rel.sys at the end: the standalone fence is a full MEMBAR.SYS that also drains this SM's outstanding stores,
-// the acquire load is not.
-__device__ __forceinline__ void wait_flag(const CommDev& c, const uint32_t* flag, uint32_t seq) {
+// Bounded wait until *flag >= seq.  Flags and sequence numbers are 64-bit and only grow (one op per increment never
+// wraps), so a plain unsigned compare is exact: a never-written (0) or stale slot is always behind.  Polls with
+// ld.acquire.sys itself rather than relaxed polling + one fence.acq_rel.sys at the end: the standalone fence is a full
+// MEMBAR.SYS that also drains this SM's outstanding stores, the acquire load is not.
+__device__ __forceinline__ void wait_flag(const CommDev& c, const uint64_t* flag, uint64_t seq) {
   unsigned long long t0 = 0;
   unsigned spins = 0;
-  while (static_cast<int32_t>(ld_acquire_sys(flag) - seq) < 0) {
+  while (ld_acquire_sys(flag) < seq) {
     if ((++spins & 63u) == 0) {
       const unsigned long long now = globaltimer_ns();
       if (t0 == 0) {
@@ -702,15 +718,15 @@ __device__ __forceinline__ void wait_wire(const CommDev& c, const uint8_t* p, Wi
 
 // ---- cross-GPU barrier among the CTAs with the same blockIdx.x on every rank --------------------
 // Thread p (< world) publishes `seq` into peer p's flag slot for this CTA index and waits for peer
-// p's `seq` in its own slot.  Sequence numbers only grow, so "flag >= seq" (wrap-safe) is the test.
-__device__ __forceinline__ void cta_xbar(const CommDev& c, uint32_t seq) {
+// p's `seq` in its own slot.  Sequence numbers only grow, so "flag >= seq" is the test.
+__device__ __forceinline__ void cta_xbar(const CommDev& c, uint64_t seq) {
   __syncthreads();  // all of this CTA's data stores are ordered before the release below
   if (threadIdx.x < c.world) {
     const int jj = threadIdx.x;  // this thread pairs with rank p = (rank + jj) % world
     const int p = rank_at(c, jj);
     const size_t slot = c.flag_off + static_cast<size_t>(blockIdx.x) * kFlagSlotBytes;
-    uint32_t* theirs = reinterpret_cast<uint32_t*>(peer_sel(c, jj) + slot) + c.rank;
-    const uint32_t* mine = reinterpret_cast<const uint32_t*>(c.peer[0] + slot) + p;
+    uint64_t* theirs = reinterpret_cast<uint64_t*>(peer_sel(c, jj) + slot) + c.rank;
+    const uint64_t* mine = reinterpret_cast<const uint64_t*>(c.peer[0] + slot) + p;
     st_release_sys(theirs, seq);
     wait_flag(c, mine, seq);
   }
@@ -720,22 +736,23 @@ __device__ __forceinline__ void cta_xbar(const CommDev& c, uint32_t seq) {
 // Every collective kernel starts by reading the communicator's op counter (parity selects the
 // staging buffer, the value seeds this op's flag sequence numbers) and ends by bumping it once
 // all CTAs are through.  Keeping the counter on the device makes the launch sequence CUDA-graph
-// replayable and keeps the host stateless.
-__device__ __forceinline__ uint32_t op_begin(const CommDev& c) { return ld_volatile_u32(c.opseq); }
+// replayable and keeps the host stateless.  The bump is an add, not a store of seq0 + 1 (nothing else
+// writes the counter while a collective runs): the 64-bit seq0 need not stay live to the end of the kernel.
+__device__ __forceinline__ uint64_t op_begin(const CommDev& c) { return ld_volatile_u64(c.opseq); }
 
 // The staging buffer of the op whose counter is seq0: consecutive ops alternate between the two.
-__device__ __forceinline__ unsigned long long stage_of(const CommDev& c, uint32_t seq0) {
+__device__ __forceinline__ unsigned long long stage_of(const CommDev& c, uint64_t seq0) {
   return (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
 }
 
-__device__ __forceinline__ void op_end(const CommDev& c, uint32_t seq0) {
+__device__ __forceinline__ void op_end(const CommDev& c) {
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
     if (atomicAdd(c.done, 1u) == gridDim.x - 1) {
       *reinterpret_cast<volatile uint32_t*>(c.done) = 0;
       __threadfence();
-      *reinterpret_cast<volatile uint32_t*>(c.opseq) = seq0 + 1;
+      atomicAdd(reinterpret_cast<unsigned long long*>(c.opseq), 1ull);
     }
   }
 }

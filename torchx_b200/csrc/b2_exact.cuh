@@ -204,7 +204,7 @@ template <int DT, int OP>
 __global__ void __launch_bounds__(kThreads, 1) k_reduce_exact(CommDev c, void* buf, unsigned long long n) {
   using namespace dev;
   constexpr int E = exact::DtypeTraits<DT>::kBytes;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   uint8_t* p = static_cast<uint8_t*>(buf);
   const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
@@ -225,7 +225,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_exact(CommDev c, void* b
       if (r < c.world) acc = exact::combine<DT, OP>(acc, q[r]);
     exact::st_local<E>(p, aligned, v, n, acc);
   }
-  op_end(c, seq0);
+  op_end(c);
 }
 
 // Rank r's `bytes` bytes land at out + r * block.  `in` may be this rank's own block (torch's in-place form): that block
@@ -233,7 +233,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_exact(CommDev c, void* b
 __global__ void __launch_bounds__(kThreads, 1)
     k_allgather(CommDev c, uint8_t* out, const uint8_t* in, unsigned long long bytes, unsigned long long block) {
   using namespace dev;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const bool in_aligned = (reinterpret_cast<uintptr_t>(in) & 15u) == 0;
   const bool in_place = in == out + static_cast<unsigned long long>(c.rank) * block;
@@ -256,5 +256,5 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
   }
-  op_end(c, seq0);
+  op_end(c);
 }

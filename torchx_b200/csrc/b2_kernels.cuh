@@ -222,7 +222,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
   if (threadIdx.x == 0) trace_stamp(c, 3);
-  op_end(c, seq0);
+  op_end(c);
 }
 
 // Two-shot, single pass: bandwidth regime for worlds / sizes the pipelined kernels do not take.  The message is cut into
@@ -292,7 +292,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
@@ -386,7 +386,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
   if (threadIdx.x == 0) trace_stamp(c, 5);
-  op_end(c, seq0);
+  op_end(c);
 }
 
 // Broadcast of raw bytes: root pushes into every peer's stage, one barrier, peers copy out.  The stage is always
@@ -396,7 +396,7 @@ __global__ void __launch_bounds__(kThreads, 1)
 __global__ void __launch_bounds__(kThreads, 1)
     k_broadcast(CommDev c, uint8_t* buf, unsigned long long bytes, int root) {
   using namespace dev;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
   const unsigned long long nvec = bytes / 16;
@@ -439,12 +439,12 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     for (unsigned long long b = nvec * 16 + first; b < bytes; b += stride) buf[b] = src[b];
   }
-  op_end(c, seq0);
+  op_end(c);
 }
 
 __global__ void __launch_bounds__(kThreads, 1) k_barrier(CommDev c) {
   using namespace dev;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   cta_xbar(c, seq0 * 4u + 1u);
-  op_end(c, seq0);
+  op_end(c);
 }

@@ -31,7 +31,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long base_ll = (seq0 & 1u) ? c.ll_off[1] : c.ll_off[0];
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
@@ -50,9 +50,10 @@ __global__ void __launch_bounds__(kThreads, 1)
     const int jj = threadIdx.x;
     const int p = slice_of<W>(c.rank, jj);
     if (blockIdx.x == 0)
-      asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(reinterpret_cast<uint32_t*>(peer_sel(c, jj) + c.llflag_off) + c.rank), "r"(seq0)
+      asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(reinterpret_cast<uint64_t*>(peer_sel(c, jj) + c.llflag_off) + c.rank), "l"(seq0)
                    : "memory");
-    if (jj != 0) wait_flag(c, reinterpret_cast<const uint32_t*>(mine + c.llflag_off) + p, seq0 - 1u);
+    // the first op has no predecessor: wait for 0, not for seq0 - 1 = 2^64 - 1
+    if (jj != 0) wait_flag(c, reinterpret_cast<const uint64_t*>(mine + c.llflag_off) + p, seq0 == 0 ? 0 : seq0 - 1);
   }
   __syncthreads();
   if (threadIdx.x == 0) trace_stamp(c, 1);
@@ -166,5 +167,5 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
   if (threadIdx.x == 0) trace_stamp(c, 5);
-  op_end(c, seq0);
+  op_end(c);
 }

@@ -63,9 +63,9 @@ __device__ __forceinline__ uint32_t mail_peek(const uint32_t* box) {
   return v;
 }
 
-__device__ __forceinline__ uint32_t* flag_slot(uint8_t* arena, const CommDev& c, int kind, int k) {
+__device__ __forceinline__ uint64_t* flag_slot(uint8_t* arena, const CommDev& c, int kind, int k) {
   const size_t idx = (static_cast<size_t>(blockIdx.x) * kPipeKinds + kind) * kMaxChunks + k;
-  return reinterpret_cast<uint32_t*>(arena + c.pflag_off + idx * kFlagSlotBytes);
+  return reinterpret_cast<uint64_t*>(arena + c.pflag_off + idx * kFlagSlotBytes);
 }
 
 // Data side: the `count` data threads of a role have issued their stores for chunk k.
@@ -79,7 +79,7 @@ __device__ __forceinline__ void chunk_done(int id, int count, int t, uint32_t* b
 // for the drain of the memory system's backlog, and fences of one warp do not overlap): the pipeline granularity
 // adapts to the fence latency instead of serialising K fences.
 template <bool FENCE>
-__device__ __forceinline__ void signaller(const CommDev& c, int lane, const uint32_t* box, int kind, int nk, uint32_t seq) {
+__device__ __forceinline__ void signaller(const CommDev& c, int lane, const uint32_t* box, int kind, int nk, uint64_t seq) {
   int k = 0;
   while (k < nk) {
     unsigned long long t0 = 0;
@@ -102,13 +102,13 @@ __device__ __forceinline__ void signaller(const CommDev& c, int lane, const uint
       if constexpr (FENCE) asm volatile("fence.acq_rel.sys;" ::: "memory");
       uint8_t* their = dev::peer_sel(c, lane);
       for (int kk = k; kk < static_cast<int>(done); ++kk)
-        asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(flag_slot(their, c, kind, kk) + c.rank), "r"(seq) : "memory");
+        asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(flag_slot(their, c, kind, kk) + c.rank), "l"(seq) : "memory");
     }
     k = static_cast<int>(done);
   }
 }
 // Wait until every rank has published `seq` for (kind, k): thread t (< world) polls word [t] of my own slot.
-__device__ __forceinline__ void group_wait(const CommDev& c, int id, int count, int t, int kind, int k, uint32_t seq) {
+__device__ __forceinline__ void group_wait(const CommDev& c, int id, int count, int t, int kind, int k, uint64_t seq) {
   if (t < c.world) dev::wait_flag(c, flag_slot(c.peer[0], c, kind, k) + t, seq);
   group_sync(id, count);  // peers' data is now visible to every thread of the group (the acquire invalidated L1)
 }
@@ -123,8 +123,8 @@ __global__ void __launch_bounds__(kThreads, 1)
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
   __shared__ uint32_t mail[2];  // [0]: chunks role A has finished, [1]: chunks role B has finished
-  const uint32_t seq0 = op_begin(c);
-  const uint32_t seq = seq0 * 4u + 1u;
+  const uint64_t seq0 = op_begin(c);
+  const uint64_t seq = seq0 * 4u + 1u;
   const unsigned long long stage = stage_of(c, seq0);
   const bool aligned = buf_aligned<MODE>(buf);
   const unsigned long long V = (n + 7) / 8;
@@ -290,5 +290,5 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     if (t == 0) trace_stamp(c, 5);
   }
-  op_end(c, seq0);
+  op_end(c);
 }

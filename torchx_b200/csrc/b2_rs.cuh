@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
   constexpr int U = vecs_per_trip(W);
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long V = (n + 7) / 8;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
   }
-  op_end(c, seq0);
+  op_end(c);
 }
 
 // The same reduce-scatter with the optimizer step as its phase B epilogue (b2_reduce_scatter_step, b2_optim.cuh): the
@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;
   __shared__ OptCta t;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   // stage_of(c, seq0), open-coded: the call moves ptxas's register allocation of 8 instances (modes 0, 1 and 3 at W <= 4)
   const unsigned long long stage = (seq0 & 1u) ? c.stage_off[1] : c.stage_off[0];
   const unsigned long long V = (n + 7) / 8;
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     const F8 s = reduce_rank_order<MODE, W>(w);
     opt_step_vec(o, t, h, v * 8, n, widen<MODE>(finalize<MODE>(s)));
   }
-  op_end(c, seq0);
+  op_end(c);
 }
 
 // Integer SUM and MIN / MAX on every dtype: out[i] <- OP over r of in_r[rank block][i], combined in rank order, on raw
@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter_exact(CommDev c,
                                                                        unsigned long long n, unsigned long long block) {
   using namespace dev;
   constexpr int E = exact::DtypeTraits<DT>::kBytes;
-  const uint32_t seq0 = op_begin(c);
+  const uint64_t seq0 = op_begin(c);
   const unsigned long long stage = stage_of(c, seq0);
   const unsigned long long V = (n * E + 15) / 16;
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * kThreads;
@@ -171,5 +171,5 @@ __global__ void __launch_bounds__(kThreads, 1) k_reduce_scatter_exact(CommDev c,
       if (r < c.world) acc = exact::combine<DT, OP>(acc, q[r]);
     exact::st_local<E>(p, aligned, v, n, acc);
   }
-  op_end(c, seq0);
+  op_end(c);
 }

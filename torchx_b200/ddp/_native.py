@@ -129,6 +129,7 @@ SIGNATURES = {
     "b2_comm_set_max_ctas": (_i, [_vp, _i]),
     "b2_comm_set_param": (_i, [_vp, ctypes.c_char_p, ctypes.c_longlong]),
     "b2_comm_status": (_i, [_vp]),
+    "b2_comm_op_count": (_u64, [_vp]),
     "b2_comm_launch_count": (_u64, [_vp]),
     "b2_comm_last_algo": (_i, [_vp]),
     "b2_auto_algo": (_i, [_i, _i, _sz, _i]),

@@ -154,7 +154,8 @@ class Communicator:
         N.check(N.lib().b2_comm_set_max_ctas(self._h, n))
 
     def set_param(self, name: str, value: int) -> None:
-        """AUTO thresholds / pipeline chunking (include/b200ddp.h: b2_comm_set_param); same value on every rank."""
+        """AUTO thresholds / pipeline chunking, and the op counter of an idle communicator (include/b200ddp.h:
+        b2_comm_set_param); same value on every rank."""
         N.check(N.lib().b2_comm_set_param(self._h, name.encode(), int(value)))
 
     @property
@@ -181,6 +182,12 @@ class Communicator:
         """Name of the algorithm the most recent multi-rank allreduce ran (what "auto" resolved to)."""
         k = int(N.lib().b2_comm_last_algo(self._h))
         return {v: n for n, v in ALGOS.items()}.get(k, "none") if k else "none"
+
+    @property
+    def op_count(self) -> int:
+        """The device op counter (b2_comm_op_count): collectives completed, plus any ``set_param("op_count", v)``.
+        Synchronous."""
+        return int(N.lib().b2_comm_op_count(self._h))
 
     @property
     def launches(self) -> int:
