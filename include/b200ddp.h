@@ -19,6 +19,7 @@
  *                         (both SUM an int64 one-hot tensor)
  *   b2_allgather       <- `dist.all_gather_into_tensor` / `dist.all_gather`
  *   b2_reduce_scatter  <- `dist.reduce_scatter_tensor` / `dist.reduce_scatter`
+ *   b2_reduce          <- `dist.reduce`
  *   b2_alltoall, b2_alltoall_max_bytes <- `dist.all_to_all_single` / `dist.all_to_all`
  *   b2_p2p             <- dist.send / dist.recv / dist.batch_isend_irecv (and the gather / scatter built on them)
  *   b2_batchnorm_stats <- torch's SyncBatchNorm forward: all_gather of (mean, invstd, count) + the count mask +
@@ -50,8 +51,8 @@ extern "C" {
 #endif
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
-                            b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats
-                            and b2_bn_backward_reduce, which only add symbols: a binding that needs them
+                            b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats,
+                            b2_bn_backward_reduce and b2_reduce, which only add symbols: a binding that needs them
                             fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -270,6 +271,15 @@ int b2_allgather(b2_comm_t* comm, void* out, const void* in, size_t bytes, void*
  * B2_EINVAL.  n_elems == 0 is a no-op; at W == 1 it copies the block (nothing if in place).  Each rank sends and
  * receives (W-1)/W of its input. */
 int b2_reduce_scatter(b2_comm_t* comm, void* out, const void* in, size_t n_elems, int dtype, int op, void* stream);
+
+/* In place on the root: buf[i] <- op_r buf_r[i] over `n_elems` elements on rank `root`; every other rank's `buf` is only
+ * read.  Same dtypes, ops and arithmetic contract as b2_allreduce_op: the root's `buf` is what b2_allreduce_op of the same
+ * inputs leaves, bit for bit, except where that allreduce's B2_ALGO_AUTO picked B2_ALGO_NVLS, and it is the concatenation
+ * of the W blocks b2_reduce_scatter leaves.  Checked in b2_allreduce_op's order: dtype and op (even when n_elems == 0),
+ * then n_elems == 0 is a no-op, then a null communicator or buffer, a root outside [0, W) (B2_EINVAL) and a poisoned
+ * communicator (B2_ESTATE).  W == 1 leaves `buf` as it is.  Each rank sends (W-1)/W of its input; the root also receives
+ * (W-1)/W of it. */
+int b2_reduce(b2_comm_t* comm, void* buf, size_t n_elems, int dtype, int op, int root, void* stream);
 
 /*
  * The gradient reduce-scatter of a sharded bucket (the mini-DDP's ZeRO-1 mode), with its input gathered from a segment

@@ -16,6 +16,7 @@
 //   * broadcast / barrier on the same fabric (DDP init + BN-buffer sync, dist.barrier()).
 //   * the exact collectives of a training script: integer SUM and MIN / MAX allreduce, all-gather (b2_exact.cuh).
 //   * reduce-scatter with the allreduce's arithmetic: push-scatter, one barrier, reduce own block (b2_rs.cuh).
+//   * reduce to a root: the reduce-scatter's reduced slices pulled by the root alone (b2_reduce.cuh).
 //   * all-to-all with any split sizes: push each block behind a count header, one barrier, copy out (b2_a2a.cuh).
 //   * point-to-point send / recv in batches: per-channel slot inboxes with flags and credits, no barrier (b2_p2p.cuh).
 //   * SyncBatchNorm's statistics exchange: gather + merge of every rank's mean / invstd / count (b2_bnstats.cuh).
@@ -35,6 +36,7 @@
 #include "b2_ll.cuh"
 #include "b2_exact.cuh"
 #include "b2_rs.cuh"
+#include "b2_reduce.cuh"
 #include "b2_a2a.cuh"
 #include "b2_p2p.cuh"
 #include "b2_bnstats.cuh"
@@ -1521,6 +1523,50 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
     return le;
   });
   if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+int b2_reduce(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, int root, void* stream) {
+  if (const int rc = check_dtype_op("b2_reduce", dtype, op)) return rc;
+  if (n_elems == 0) return B2_OK;
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  if (!buf) return fail(B2_EINVAL, "b2_reduce: null buffer");
+  const int W = c->d.world;
+  if (root < 0 || root >= W) return fail(B2_EINVAL, "b2_reduce: root %d is not a rank of a world of %d", root, W);
+  if (const int rc = check_not_poisoned(c)) return rc;
+  if (W == 1) return B2_OK;
+  DeviceGuard g(c->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool sum = !dtype_is_int(dtype) && (op == B2_OP_SUM || op == B2_OP_AVG);
+  const int mode = sum_mode_for(dtype);
+  const size_t eb = dtype_bytes(dtype);
+  // the two-shot allreduce's plan: a launch holds W slices of at most one recv region each (whole vecs in either case)
+  const size_t cap = sum ? c->d.slice_cap / wire_vec_bytes(mode) * 8 * W : c->d.slice_cap / 16 * W * (16 / eb);
+  const float scale = op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f;
+  uint8_t* p = static_cast<uint8_t*>(buf);
+  const cudaError_t e = for_chunks(c, n_elems, cap, [&](size_t off, size_t n) {
+    cudaError_t le = cudaErrorInvalidValue;  // never guess a mode
+    if (sum) {
+      const unsigned long long Ls = ((n + 7) / 8 + W - 1) / W;
+      with_mode(mode, [&](auto m) {
+        constexpr int MODE = decltype(m)::value;
+        if constexpr (MODE == B2_F32 || MODE == B2_BF16 || MODE == B2_F16) {  // the modes sum_mode_for picks
+          with_world(W, [&](auto w) {
+            k_reduce<MODE, decltype(w)::value><<<grid_for(c, Ls, vecs_per_trip(W)), kThreads, 0, s>>>(c->d, p + off * eb, n, scale, root);
+            le = cudaGetLastError();
+          });
+        }
+      });
+    } else {
+      const unsigned long long Ls = ((n * eb + 15) / 16 + W - 1) / W;
+      with_exact_op(dtype, op, [&](auto dt, auto oc) {
+        k_reduce_exact_root<decltype(dt)::value, decltype(oc)::value><<<grid_for(c, Ls, 1), kThreads, 0, s>>>(c->d, p + off * eb, n, root);
+        le = cudaGetLastError();
+      });
+    }
+    return le;
+  });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "reduce kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 

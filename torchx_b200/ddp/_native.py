@@ -140,6 +140,7 @@ SIGNATURES = {
     "b2_allreduce_op": (_i, [_vp, _vp, _sz, _i, _i, _vp]),
     "b2_allgather": (_i, [_vp, _vp, _vp, _sz, _vp]),
     "b2_reduce_scatter": (_i, [_vp, _vp, _vp, _sz, _i, _i, _vp]),
+    "b2_reduce": (_i, [_vp, _vp, _sz, _i, _i, _i, _vp]),
     "b2_reduce_scatter_gather": (_i, [_vp, _vp, _sz, _P(B2Segment), _i, _i, _f, _vp]),
     "b2_reduce_scatter_step": (_i, [_vp, _sz, _P(B2Segment), _i, _i, _f, _P(B2Optim), _vp]),
     "b2_alltoall": (_i, [_vp, _P(_vp), _P(_sz), _P(_vp), _P(_sz), _vp]),

@@ -268,6 +268,19 @@ class Communicator:
                                           code, _stream_arg(stream, self.device)))
         return out
 
+    def reduce_(self, t: torch.Tensor, root: int, op: str = "sum", stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+        """On rank ``root``, in place, ``t <- op over ranks of t``; every other rank's ``t`` is only read (include/b200ddp.h:
+        b2_reduce).  The root ends with the bits ``allreduce_op_`` leaves wherever that allreduce sums in rank order (every
+        algorithm but NVLS); each rank sends (W-1)/W of ``t`` and only the root takes the reduced slices back in."""
+        dt, code = dtype_op_for(t.dtype, op, "reduce_")
+        r = as_rank(root)
+        if r is None or not 0 <= r < self.world:
+            raise ValueError(f"reduce_: root {root!r} is not a rank of a world of {self.world}")
+        self._check_tensor(t)
+        N.check(N.lib().b2_reduce(self._h, ctypes.c_void_p(t.data_ptr()), t.numel(), dt, code, r,
+                                  _stream_arg(stream, self.device)))
+        return t
+
     def reduce_scatter_gather_(self, out: torch.Tensor, segments, n_segments: int, scale: Optional[float] = None,
                                wire: str = "bf16", stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
         """``out`` (``block`` elements) <- block ``rank`` of ``allreduce_gather_`` over the padded bucket of ``world * block``

@@ -9,11 +9,15 @@ environment contract and barrier-ordered critical sections.  Two backends behind
   * ``init_pg("b200")`` - the peer-buffer communicator from ``libb200ddp.so``: no TCP store, no NCCL.  ``barrier`` /
     ``on_rank0_first``, ``all_reduce``, ``all_gather_into_tensor``, ``all_gather``, ``reduce_scatter_tensor``,
     ``reduce_scatter``, ``broadcast``, ``all_to_all_single``, ``all_to_all``, the point-to-point ``send``, ``recv``,
-    ``isend``, ``irecv``, ``P2POp`` / ``batch_isend_irecv``, and ``gather`` / ``scatter`` then run on that fabric.
+    ``isend``, ``irecv``, ``P2POp`` / ``batch_isend_irecv``, ``gather`` / ``scatter``, ``reduce`` to a root and the object
+    collectives ``all_gather_object``, ``broadcast_object_list``, ``gather_object``, ``scatter_object_list``,
+    ``send_object_list`` / ``recv_object_list`` then run on that fabric.  The object collectives unpickle what peers send,
+    so they trust every peer, as torch's do.
 """
 from __future__ import annotations
 
 import os
+import pickle
 import warnings
 from contextlib import contextmanager
 from typing import Any, Iterator, List, Optional
@@ -425,6 +429,224 @@ def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor) -> N
     for t in tensors:
         if t.dtype != like.dtype or t.numel() != like.numel():
             raise ValueError(f"{what}: every tensor must be {like.dtype} with {like.numel()} elements")
+
+
+def reduce(tensor: torch.Tensor, dst: int, op: Any = dist.ReduceOp.SUM, group: Any = None, async_op: bool = False) -> Any:
+    """``torch.distributed.reduce`` in place: on rank ``dst``, ``tensor`` <- the reduction over ranks of ``tensor``; every
+    other rank's ``tensor`` is only read.  Under ``init_pg("b200")`` rank ``dst`` ends with the bits ``all_reduce`` with the
+    same op leaves (include/b200ddp.h: b2_reduce), and each rank sends (W-1)/W of the tensor."""
+    if not _on_fabric():
+        return dist.reduce(tensor, dst, op=op, group=group, async_op=async_op)
+    _check_native_call(group, async_op)
+    dst = _check_rank("reduce: dst", dst)
+    _COMM.reduce_(tensor, dst, reduce_op_name(op))
+    return None
+
+
+# ---- object collectives ----------------------------------------------------------------------------------------------
+# On the fabric each one pickles every object into a uint8 tensor on the communicator's device, exchanges the int64 sizes,
+# then the bytes (padded to the largest size where the exchange needs equal blocks), and unpickles on the host: two fabric
+# operations and one device-to-host copy per call, as torch's are.  Unpickling runs whatever the bytes say: these calls
+# trust every peer, exactly as torch's do.
+
+
+def _comm_device() -> torch.device:
+    return torch.device("cuda", _COMM.device)
+
+
+def _check_object_call(fn: str, group: Any, device: Any = None) -> torch.device:
+    """The device an object collective runs on: the communicator's.  ``group`` must be None or WORLD and ``device``, if
+    given, the communicator's device: the fabric never moves the exchange elsewhere."""
+    _check_native_call(group, False)
+    here = _comm_device()
+    if device is not None:
+        d = torch.device(device)
+        if d.type == "cuda" and d.index is None:
+            d = torch.device("cuda", torch.cuda.current_device())
+        if d != here:
+            raise ValueError(f"{fn}: device {device} is not the b200 communicator's device {here}")
+    return here
+
+
+def _peer_arg(fn: str, name: str, r: Any, group_r: Any, default: Optional[int] = 0) -> int:
+    """``src`` / ``dst`` of an object collective; ``group_src`` / ``group_dst`` may stand in for it or repeat it (with no
+    subgroups the group rank is the rank)."""
+    if group_r is not None:
+        if r is not None and r != group_r:
+            raise ValueError(f"{fn}: group_{name} {group_r!r} differs from {name} {r!r}; the b200 communicator has no subgroups")
+        r = group_r
+    if r is None:
+        if default is None:
+            raise ValueError(f"{fn}: {name} must be given")
+        r = default
+    return _check_rank(f"{fn}: {name}", r)
+
+
+def _to_bytes(obj: Any, device: torch.device) -> torch.Tensor:
+    data = pickle.dumps(obj)
+    return torch.frombuffer(bytearray(data), dtype=torch.uint8).to(device)
+
+
+def _padded(t: torch.Tensor, size: int) -> torch.Tensor:
+    out = torch.zeros(size, dtype=torch.uint8, device=t.device)
+    out[: t.numel()] = t
+    return out
+
+
+def _concat_sizes(tensors: List[torch.Tensor], device: torch.device):
+    sizes = torch.tensor([t.numel() for t in tensors], dtype=torch.int64).to(device)
+    return sizes, (torch.cat(tensors) if len(tensors) != 1 else tensors[0])
+
+
+def _split_objects(object_list: List[Any], sizes: List[int], data: torch.Tensor) -> None:
+    host = data.cpu().numpy().tobytes()
+    at = 0
+    for i, n in enumerate(sizes):
+        object_list[i] = pickle.loads(host[at: at + n])
+        at += n
+
+
+def all_gather_object(object_list: List[Any], obj: Any, group: Any = None) -> None:
+    """``torch.distributed.all_gather_object``: ``object_list[r]`` <- rank r's ``obj`` (any picklable object).  Under
+    ``init_pg("b200")``: one all-gather of the sizes, one of the padded bytes.  Unpickling trusts every peer."""
+    if not _on_fabric():
+        return dist.all_gather_object(object_list, obj, group=group)
+    device = _check_object_call("all_gather_object", group)
+    W = _COMM.world
+    mine = _to_bytes(obj, device)
+    sizes = torch.empty(W, dtype=torch.int64, device=device)
+    _COMM.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
+    sizes = sizes.tolist()
+    block = max(sizes)
+    out = torch.empty(W * block, dtype=torch.uint8, device=device)
+    _COMM.allgather_(out, _padded(mine, block))
+    host = out.cpu().numpy().tobytes()
+    for r in range(W):
+        object_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
+    return None
+
+
+def gather_object(obj: Any, object_gather_list: Optional[List[Any]] = None, dst: Optional[int] = None, group: Any = None,
+                  group_dst: Optional[int] = None) -> None:
+    """``torch.distributed.gather_object``: on rank ``dst`` (default 0), ``object_gather_list[r]`` <- rank r's ``obj``; the
+    other ranks pass no list.  Under ``init_pg("b200")``: an all-gather of the sizes, then ``gather`` of the padded bytes.
+    Unpickling trusts every peer."""
+    if not _on_fabric():
+        return dist.gather_object(obj, object_gather_list, dst=dst, group=group, group_dst=group_dst)
+    device = _check_object_call("gather_object", group)
+    dst = _peer_arg("gather_object", "dst", dst, group_dst)
+    if _COMM.rank == dst and not object_gather_list:
+        raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
+    if _COMM.rank != dst and object_gather_list:
+        raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
+    W = _COMM.world
+    mine = _to_bytes(obj, device)
+    sizes = torch.empty(W, dtype=torch.int64, device=device)
+    _COMM.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
+    sizes = sizes.tolist()
+    block = max(sizes)
+    if _COMM.rank != dst:
+        gather(_padded(mine, block), None, dst=dst)
+        return None
+    out = torch.empty(W, block, dtype=torch.uint8, device=device)
+    gather(_padded(mine, block), list(out.unbind(0)), dst=dst)
+    host = out.cpu().numpy().tobytes()
+    for r in range(W):
+        object_gather_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
+    return None
+
+
+def broadcast_object_list(object_list: List[Any], src: Optional[int] = None, group: Any = None, device: Any = None,
+                          group_src: Optional[int] = None) -> None:
+    """``torch.distributed.broadcast_object_list``: every rank's ``object_list`` (of one length on every rank) <- rank
+    ``src``'s (default 0), in place; ``src``'s list is left as it is.  Under ``init_pg("b200")``: one broadcast of the
+    sizes, one of the concatenated bytes.  Unpickling trusts rank ``src``."""
+    if not _on_fabric():
+        return dist.broadcast_object_list(object_list, src=src, group=group, device=device, group_src=group_src)
+    dev = _check_object_call("broadcast_object_list", group, device)
+    src = _peer_arg("broadcast_object_list", "src", src, group_src)
+    if _COMM.rank == src:
+        sizes, data = _concat_sizes([_to_bytes(o, dev) for o in object_list], dev)
+        _COMM.broadcast_(sizes, root=src)
+        _COMM.broadcast_(data, root=src)
+        return None
+    sizes = torch.empty(len(object_list), dtype=torch.int64, device=dev)
+    _COMM.broadcast_(sizes, root=src)
+    sizes = sizes.tolist()
+    data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
+    _COMM.broadcast_(data, root=src)
+    _split_objects(object_list, sizes, data)
+    return None
+
+
+def scatter_object_list(scatter_object_output_list: List[Any], scatter_object_input_list: Optional[List[Any]] = None,
+                        src: Optional[int] = None, group: Any = None, group_src: Optional[int] = None) -> None:
+    """``torch.distributed.scatter_object_list``: every rank r's ``scatter_object_output_list[0]`` <- rank ``src``'s
+    (default 0) ``scatter_object_input_list[r]``.  Under ``init_pg("b200")``: one broadcast of the W sizes, then
+    ``scatter`` of the padded bytes.  Unpickling trusts rank ``src``."""
+    if not _on_fabric():
+        return dist.scatter_object_list(scatter_object_output_list, scatter_object_input_list, src=src, group=group,
+                                        group_src=group_src)
+    device = _check_object_call("scatter_object_list", group)
+    src = _peer_arg("scatter_object_list", "src", src, group_src)
+    if not isinstance(scatter_object_output_list, list) or len(scatter_object_output_list) < 1:
+        raise ValueError("Expected argument scatter_object_output_list to be a list of size at least 1.")
+    W = _COMM.world
+    if _COMM.rank == src:
+        if scatter_object_input_list is None:
+            raise ValueError("source rank must provide non-None scatter_object_input_list")
+        if len(scatter_object_input_list) != W:
+            raise ValueError(f"scatter_object_list: scatter_object_input_list has {len(scatter_object_input_list)} objects, "
+                             f"world size is {W}")
+        parts = [_to_bytes(o, device) for o in scatter_object_input_list]
+        _COMM.broadcast_(torch.tensor([t.numel() for t in parts], dtype=torch.int64).to(device), root=src)
+        block = max(t.numel() for t in parts)
+        out = torch.empty(block, dtype=torch.uint8, device=device)
+        scatter(out, [_padded(t, block) for t in parts], src=src)
+        n = parts[src].numel()
+    else:
+        sizes = torch.empty(W, dtype=torch.int64, device=device)
+        _COMM.broadcast_(sizes, root=src)
+        sizes = sizes.tolist()
+        out = torch.empty(max(sizes), dtype=torch.uint8, device=device)
+        scatter(out, None, src=src)
+        n = sizes[_COMM.rank]
+    scatter_object_output_list[0] = pickle.loads(out[:n].cpu().numpy().tobytes())
+    return None
+
+
+def send_object_list(object_list: List[Any], dst: Optional[int] = None, group: Any = None, device: Any = None,
+                     group_dst: Optional[int] = None, use_batch: bool = False) -> None:
+    """``torch.distributed.send_object_list``: rank ``dst`` receives ``object_list`` with ``recv_object_list``.  Under
+    ``init_pg("b200")``: one send of the sizes, one of the concatenated bytes; ``use_batch`` is accepted and ignored."""
+    if not _on_fabric():
+        return dist.send_object_list(object_list, dst=dst, group=group, device=device, group_dst=group_dst, use_batch=use_batch)
+    dev = _check_object_call("send_object_list", group, device)
+    dst = _peer_arg("send_object_list", "dst", dst, group_dst, default=None)
+    sizes, data = _concat_sizes([_to_bytes(o, dev) for o in object_list], dev)
+    _COMM.p2p_([("send", sizes, dst)])
+    _COMM.p2p_([("send", data, dst)])
+    return None
+
+
+def recv_object_list(object_list: List[Any], src: Optional[int] = None, group: Any = None, device: Any = None,
+                     group_src: Optional[int] = None, use_batch: bool = False) -> int:
+    """``torch.distributed.recv_object_list``: ``object_list`` (as long as the sender's) <- the objects rank ``src`` sends
+    with ``send_object_list``, in place; returns ``src``.  Receiving from any rank is not available on the fabric.
+    Unpickling trusts rank ``src``."""
+    if not _on_fabric():
+        return dist.recv_object_list(object_list, src=src, group=group, device=device, group_src=group_src, use_batch=use_batch)
+    dev = _check_object_call("recv_object_list", group, device)
+    if src is None and group_src is None:
+        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
+    src = _peer_arg("recv_object_list", "src", src, group_src)
+    sizes = torch.empty(len(object_list), dtype=torch.int64, device=dev)
+    _COMM.p2p_([("recv", sizes, src)])
+    sizes = sizes.tolist()
+    data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
+    _COMM.p2p_([("recv", data, src)])
+    _split_objects(object_list, sizes, data)
+    return src
 
 
 @contextmanager
