@@ -221,8 +221,13 @@ int b2_allreduce(b2_comm_t* comm, void* buf, size_t n_elems, int mode, float sca
  * [begin, end) and reads them from the DEVICE pointer `src` (this rank's tensor of the bucket's dtype, dense in the
  * bucket's element order; it may alias `out`).  The table is copied into the kernel parameters by this call: it need not
  * outlive it.  `out` is this rank's bucket.  More parameters than B2_MAX_SEGMENTS: B2_EINVAL (copy in, then b2_allreduce).
+ * A segment whose `src` is B2_SEGMENT_ZEROS contributes +0.0 for each of its elements, exactly as a zero-filled tensor of
+ * the bucket's dtype would, and is not read from memory (a parameter that got no gradient in this step).  A NULL `src`
+ * is B2_EINVAL.
  */
 #define B2_MAX_SEGMENTS 128
+/* The `src` of a zero segment: not NULL, and misaligned for every element type, so no tensor has it. */
+#define B2_SEGMENT_ZEROS ((const void*)1)
 typedef struct b2_segment {
   const void* src;
   uint64_t begin;
@@ -286,7 +291,7 @@ int b2_reduce(b2_comm_t* comm, void* buf, size_t n_elems, int dtype, int op, int
  * table as in b2_allreduce_gather:
  *      out[i] <- round( sum_r wire( scale * segment_r(rank*block + i) ) ),   i in [0, block)
  * The table covers the padded bucket [0, W*block) in bucket order without gaps, with the rules and error texts of
- * b2_allreduce_gather; `mode` is any of the five B2_* gradient modes.  out[0, block) is this rank's block of what
+ * b2_allreduce_gather, B2_SEGMENT_ZEROS included; `mode` is any of the five B2_* gradient modes.  out[0, block) is this rank's block of what
  * b2_allreduce_gather of the same table leaves, bit for bit, wherever that allreduce runs a rank-order kernel (every
  * algorithm but B2_ALGO_NVLS).  An unknown mode is B2_EINVAL; block == 0 is a no-op; a poisoned communicator is
  * B2_ESTATE.  At W == 1 the call is the local pass of b2_allreduce_gather, with its rounding.  Each rank sends and
@@ -302,6 +307,7 @@ int b2_reduce_scatter_gather(b2_comm_t* comm, void* out, size_t block, const b2_
  * _fused_adamw_; fp32 parameters, no grad scale, no amsgrad):
  *      g[i] = round( sum_r wire( scale * segment_r(rank*block + i) ) )   (what b2_reduce_scatter_gather stores)
  *      param[i], state[i] <- step(group of i, param[i], g[i], state[i]),  i in [0, block)
+ * The segment table takes B2_SEGMENT_ZEROS segments as b2_reduce_scatter_gather's does.
  * `opt->param`, `opt->state0` and `opt->state1` point at `block` fp32 elements each: this rank's block of the parameter
  * buffer, then momentum_buffer (SGD) or exp_avg and exp_avg_sq (Adam / AdamW).  The runs of `opt` assign block elements to
  * parameter groups: run k covers block elements [run_begin[k], run_begin[k+1]) (run_begin[0] == 0, increasing,

@@ -1164,7 +1164,8 @@ int b2_allreduce(b2_comm_t* c, void* buf, size_t n_elems, int mode, float scale,
 }
 
 // The segment table of a gather call -> `src`: 1..B2_MAX_SEGMENTS entries that cover bucket elements [0, n_elems) in
-// order and without gaps, each with a source pointer.  `fn` names the call in the error texts.
+// order and without gaps, each with a source pointer or B2_SEGMENT_ZEROS, which the device table holds as a null pointer
+// (load_src reads such a segment as +0.0).  `fn` names the call in the error texts.
 static int segment_table(const char* fn, const b2_segment_t* segments, int n_segments, size_t n_elems, Src& src) {
   if (!segments || n_segments <= 0 || n_segments > B2_MAX_SEGMENTS)
     return fail(B2_EINVAL, "%s: need 1..%d segments (got %d)", fn, B2_MAX_SEGMENTS, n_segments);
@@ -1174,7 +1175,7 @@ static int segment_table(const char* fn, const b2_segment_t* segments, int n_seg
   for (int i = 0; i < n_segments; ++i) {
     if (segments[i].begin != at || segments[i].end <= at || !segments[i].src)
       return fail(B2_EINVAL, "%s: segment %d does not continue the bucket at element %llu", fn, i, at);
-    src.ptr[i] = segments[i].src;
+    src.ptr[i] = segments[i].src == B2_SEGMENT_ZEROS ? nullptr : segments[i].src;
     src.begin[i] = at;
     at = segments[i].end;
   }

@@ -604,16 +604,21 @@ __device__ __forceinline__ F8 load_src(const Src& src, SegHint& hint, const void
     hint.sb = sb;
     hint.se = se;
   }
+  // A null pointer is a zero segment (B2_SEGMENT_ZEROS): its elements read as +0.0 without a load.  The address is formed
+  // as an integer so that a zero segment never becomes arithmetic on a null pointer.
   const Elem* base = static_cast<const Elem*>(src.ptr[s]);
-  const Elem* p = base + (ge - sb);
-  F8 x;
-  if (e + 8 <= n && ge + 8 <= se && (reinterpret_cast<uintptr_t>(p) & (8u * sizeof(Elem) - 1u)) == 0) {
-    if constexpr (k16BitBucket<MODE>) {
-      Wire<MODE> w;
-      w.q = ldg_u4(p);
-      x = widen<MODE>(w);
-    } else {
-      x = ldg_f8(p);
+  const uintptr_t a = reinterpret_cast<uintptr_t>(base) + (ge - sb) * sizeof(Elem);
+  F8 x = {};
+  if (e + 8 <= n && ge + 8 <= se && (a & (8u * sizeof(Elem) - 1u)) == 0) {
+    if (base) {
+      const Elem* p = reinterpret_cast<const Elem*>(a);
+      if constexpr (k16BitBucket<MODE>) {
+        Wire<MODE> w;
+        w.q = ldg_u4(p);
+        x = widen<MODE>(w);
+      } else {
+        x = ldg_f8(p);
+      }
     }
   } else {  // the vec straddles parameters, is not 32 B-aligned in its tensor, or is the ragged tail
 #pragma unroll
@@ -627,7 +632,7 @@ __device__ __forceinline__ F8 load_src(const Src& src, SegHint& hint, const void
           se = src.begin[s + 1];
           base = static_cast<const Elem*>(src.ptr[s]);
         }
-        v = elem_to_f32<MODE>(base[g - sb]);
+        if (base) v = elem_to_f32<MODE>(base[g - sb]);
       }
       x.v[i] = v;
     }

@@ -68,6 +68,7 @@ NVCC_FLAGS = [
 ]
 
 B2_MAX_SEGMENTS = 128
+B2_SEGMENT_ZEROS = 1  # a segment's src: its elements read as +0.0 (a parameter without a gradient this step)
 
 
 class B2Segment(ctypes.Structure):

@@ -218,7 +218,8 @@ class Communicator:
         """``out <- round(sum_r wire(scale * concat(segments_r)))``: the bucket is only written; the input is read
         straight from the tensors the segment table points at (include/b200ddp.h: b2_allreduce_gather).  ``segments`` is a
         ctypes array of ``_native.B2Segment`` (device pointer, begin, end) covering the bucket in order; it is copied into
-        the kernel parameters by the call."""
+        the kernel parameters by the call.  A segment whose pointer is ``_native.B2_SEGMENT_ZEROS`` reads as +0.0, here and
+        in ``reduce_scatter_gather_`` / ``reduce_scatter_step_``."""
         self._check_tensor(out)
         N.check(N.lib().b2_allreduce_gather(self._h, ctypes.c_void_p(out.data_ptr()), out.numel(), segments, n_segments, mode_for(out, wire),
                                             self._scale(scale), ALGOS[algo], _stream_arg(stream, self.device)))

@@ -17,8 +17,10 @@ a 1 MiB first bucket, per-forward buffer broadcast, ``no_sync``, ``module.``-pre
 """
 from __future__ import annotations
 
+import array
 import contextlib
-from typing import Dict, Iterator, List, Optional
+import dataclasses
+from typing import Dict, Iterator, List, Optional, Set
 
 import torch
 from torch import nn
@@ -43,6 +45,44 @@ def _view_like(flat_slice: torch.Tensor, p: torch.Tensor) -> torch.Tensor:
     if p.is_contiguous() or not _dense_non_overlapping(p):
         return flat_slice.view(p.shape)
     return flat_slice.as_strided(p.shape, p.stride())
+
+
+def _find_tensors(obj) -> List[torch.Tensor]:
+    """The tensors of a forward's output, looked for where torch's DDP looks: tensors, and the items of lists, tuples, dict
+    values and dataclass fields, nested."""
+    if isinstance(obj, torch.Tensor):
+        return [obj]
+    if isinstance(obj, (list, tuple)):
+        return [t for o in obj for t in _find_tensors(o)]
+    if isinstance(obj, dict):
+        return [t for o in obj.values() for t in _find_tensors(o)]
+    if dataclasses.is_dataclass(obj) and not isinstance(obj, type):
+        return [t for f in dataclasses.fields(obj) for t in _find_tensors(getattr(obj, f.name))]
+    return []
+
+
+def _reached_leaves(outputs: List[torch.Tensor]) -> Set[int]:
+    """ids of the leaf tensors whose gradient the autograd graph of ``outputs`` accumulates: every AccumulateGrad node
+    reachable from their ``grad_fn`` through ``next_functions`` (reducer.cpp search_unused_parameters), plus outputs that
+    are themselves leaves requiring a gradient."""
+    reached: Set[int] = set()
+    stack = []
+    for t in outputs:
+        if t.grad_fn is not None:
+            stack.append(t.grad_fn)
+        elif t.requires_grad:
+            reached.add(id(t))
+    seen = set()
+    while stack:
+        fn = stack.pop()
+        if fn in seen:
+            continue
+        seen.add(fn)
+        leaf = getattr(fn, "variable", None)  # AccumulateGrad
+        if leaf is not None:
+            reached.add(id(leaf))
+        stack.extend(nxt for nxt, _ in fn.next_functions if nxt is not None and nxt not in seen)
+    return reached
 
 
 class _Bucket:
@@ -106,6 +146,8 @@ class _Bucket:
 
 
 class DistributedDataParallel(nn.Module):
+    find_unused_parameters = False  # the constructor's keyword; a class default, so an instance built without __init__ has it
+
     def __init__(
         self,
         module: nn.Module,
@@ -116,6 +158,7 @@ class DistributedDataParallel(nn.Module):
         broadcast_buffers: bool = True,
         algo: str = "auto",
         zero_copy: bool = True,
+        find_unused_parameters: bool = False,
     ) -> None:
         super().__init__()
         self.module = module
@@ -160,10 +203,23 @@ class DistributedDataParallel(nn.Module):
         self.copied_in_buckets = 0   # buckets that needed the multi-tensor copy-in (zero-copy not applicable), for tests / bench
         self.gathered_buckets = 0    # buckets whose gradients were read in place by the kernel
         self.sharded = False         # ZeRO-1 layout (ZeroRedundancyOptimizer): each rank keeps one block of every bucket
-        self._shard_grads: List = []  # (optimizer view, its gradient shard view): attached after every synced backward
+        self._shard_grads: List = []  # (optimizer view, its gradient shard view, parameter): attached after every synced backward
         self._shard_grads_live = False  # the shards hold a reduced gradient that zero_grad() has not cleared
         self._step_in_backward = None  # a ZeroRedundancyOptimizer(overlap_with_ddp=True): each bucket launch steps it
         self._synced_backwards = 0
+        # find_unused_parameters (torch's Reducer semantics, DESIGN.md 2.5): the parameters the last synced forward's output
+        # does not reach are marked ready at the first gradient hook and contribute zeros; an int32 map of the parameters
+        # whose hook fired since the last synced backward is MAX-reduced after the last bucket, and the ones no rank used
+        # keep their .grad
+        self.find_unused_parameters = find_unused_parameters
+        if find_unused_parameters:
+            self._index_of = {id(p): i for i, p in enumerate(self._params)}
+            self._unused: List[nn.Parameter] = []  # this iteration's, from the graph walk of the synced forward
+            self._unused_ids: Set[int] = set()
+            self._locally_used = array.array("i", bytes(4 * len(self._params)))
+            self._used_dev = torch.zeros(len(self._params), dtype=torch.int32, device=self.device)
+            self._used_host = torch.zeros(len(self._params), dtype=torch.int32).pin_memory()
+            self._used_event = torch.cuda.Event()
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad_ready) for p in self._params]
         # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen
         from torchx_b200.nn.bn2d import convert_batchnorm
@@ -231,12 +287,18 @@ class DistributedDataParallel(nn.Module):
             b.pending, b.ready, b.launched = len(b.params), False, False
 
     def forward(self, *args, **kwargs):
-        if torch.is_grad_enabled() and self.require_backward_grad_sync:
+        synced = torch.is_grad_enabled() and self.require_backward_grad_sync
+        if synced:
             # a kernel that gave up on a stalled peer leaves undefined bucket contents: never train on them
             self.comm.check()
             self._reset_reducer_state()
             self._sync_buffers()
-        return self.module(*args, **kwargs)
+        out = self.module(*args, **kwargs)
+        if synced and self.find_unused_parameters:  # not under no_sync, as in torch
+            reached = _reached_leaves(_find_tensors(out))
+            self._unused = [p for p in self._params if id(p) not in reached]
+            self._unused_ids = {id(p) for p in self._unused}
+        return out
 
     @contextlib.contextmanager
     def no_sync(self) -> Iterator[None]:
@@ -248,11 +310,23 @@ class DistributedDataParallel(nn.Module):
             self.require_backward_grad_sync = old
 
     def _on_grad_ready(self, p: nn.Parameter) -> None:
+        if self.find_unused_parameters:
+            self._locally_used[self._index_of[id(p)]] = 1  # no_sync backwards count too
         if not self.require_backward_grad_sync:
             return
         if not self._callback_queued:
             self._callback_queued = True
             torch.autograd.Variable._execution_engine.queue_callback(self._finalize_backward)
+            if self.find_unused_parameters:
+                for q in self._unused:
+                    self._mark_ready(q)
+        if self.find_unused_parameters and id(p) in self._unused_ids:
+            raise RuntimeError(
+                "a parameter that the forward's output does not reach produced a gradient: it was already marked ready as "
+                "unused.  Compute the loss only from the DistributedDataParallel output")
+        self._mark_ready(p)
+
+    def _mark_ready(self, p: nn.Parameter) -> None:
         b = self._bucket_of[id(p)]
         b.pending -= 1
         if b.pending == 0:
@@ -261,12 +335,27 @@ class DistributedDataParallel(nn.Module):
             while self._next_bucket < len(self.buckets) and self.buckets[self._next_bucket].ready:
                 self._launch(self.buckets[self._next_bucket])
                 self._next_bucket += 1
+            if self.find_unused_parameters and self._next_bucket == len(self.buckets):
+                self._reduce_used_map()
+
+    def _reduce_used_map(self) -> None:
+        """After the last bucket: MAX of the locally used maps on the comm stream, copied into pinned host memory.  Every
+        rank issues it, whether or not it needs the result (_finalize_backward waits only if some parameter is locally
+        unused)."""
+        with torch.cuda.stream(self._comm_stream):
+            # pageable source: the copy has taken the map's bytes when it returns, so the hooks may write it again
+            self._used_dev.copy_(torch.frombuffer(self._locally_used, dtype=torch.int32), non_blocking=True)
+            self.comm.allreduce_op_(self._used_dev, "max", stream=self._comm_stream)
+            self._used_host.copy_(self._used_dev, non_blocking=True)
+            self._used_event.record(self._comm_stream)
 
     def _gatherable(self, b: _Bucket, grads: List[torch.Tensor]) -> bool:
         """The kernel can read a gradient in place when its memory order IS the bucket's element order: same dtype,
         same (dense) strides as the bucket view the parameter's layout produced."""
         dt = b.dtype
         for g, st in zip(grads, b.view_strides):
+            if g is None:  # an unused parameter: a zero segment
+                continue
             if g.dtype != dt or not g.is_cuda or tuple(s_ for s_, z in zip(g.stride(), g.shape) if z != 1) != st:
                 return False
         return True
@@ -275,25 +364,29 @@ class DistributedDataParallel(nn.Module):
         grads = []
         for p in b.params:
             g = p.grad
-            if g is None:
+            if g is None and not self.find_unused_parameters:
                 raise RuntimeError("a parameter finished backward without a gradient (unused parameters are not supported)")
-            grads.append(g)
+            grads.append(g)  # None: an unused parameter without a gradient, which contributes zeros
         gather = self.zero_copy and b.segments is not None and self._gatherable(b, grads)
         if self.sharded:
             self._launch_shard(b, grads, gather)
             return
         if not gather:
-            src, dst = [], []
+            src, dst, zeros = [], [], []
             for g, v in zip(grads, b.views):
-                if g.data_ptr() != v.data_ptr():
+                if g is None:
+                    zeros.append(v)
+                elif g.data_ptr() != v.data_ptr():
                     src.append(g)
                     dst.append(v)
             if src:
                 torch._foreach_copy_(dst, src)
+            if zeros:
+                torch._foreach_zero_(zeros)  # the Reducer's bucket_view.zero_()
             self.copied_in_buckets += 1
         else:
             for seg, g in zip(b.segments, grads):
-                seg.src = g.data_ptr()
+                seg.src = N.B2_SEGMENT_ZEROS if g is None else g.data_ptr()
             self.gathered_buckets += 1
         cur = torch.cuda.current_stream(self.device)
         self._ready_event.record(cur)
@@ -336,12 +429,16 @@ class DistributedDataParallel(nn.Module):
         if gather:
             segs = b.segments
             for seg, g in zip(segs, grads):
-                seg.src = g.data_ptr()
+                seg.src = N.B2_SEGMENT_ZEROS if g is None else g.data_ptr()
             self.gathered_buckets += 1
         else:
             b.scratch = torch.empty(b.spec.numel, dtype=b.dtype, device=self.device)
             views = [_view_like(b.scratch[o : o + n], p) for o, n, p in zip(b.spec.offsets, b.spec.numels, b.params)]
-            torch._foreach_copy_(views, grads)
+            dst = [v for v, g in zip(views, grads) if g is not None]
+            if dst:
+                torch._foreach_copy_(dst, [g for g in grads if g is not None])
+            if len(dst) < len(views):
+                torch._foreach_zero_([v for v, g in zip(views, grads) if g is None])
             segs = b.copy_segments
             segs[0].src = b.scratch.data_ptr()
             self.copied_in_buckets += 1
@@ -372,7 +469,12 @@ class DistributedDataParallel(nn.Module):
                 missing = [b.spec.index for b in self.buckets if not b.launched]
                 raise RuntimeError(
                     f"backward finished but buckets {missing} never became ready: some parameters received no gradient "
-                    "(find_unused_parameters is not supported on this path)")
+                    + ("although the forward's output reaches them" if self.find_unused_parameters else
+                       "(find_unused_parameters is not supported on this path)"))
+            unused: Set[int] = set()  # ids of the parameters no rank used: their .grad stays as it was
+            if self.find_unused_parameters and not all(self._locally_used):
+                self._used_event.synchronize()  # used on every rank when used here: only then is the reduced map needed
+                unused = {id(p) for p, u in zip(self._params, self._used_host.tolist()) if not u}
             cur = torch.cuda.current_stream(self.device)
             for b in self.buckets:
                 cur.wait_event(b.done)
@@ -382,9 +484,11 @@ class DistributedDataParallel(nn.Module):
                         p.grad = None  # frees the full-size gradients: the reduced ones exist only as the shards
                 else:
                     for p, v in zip(b.params, b.views):
-                        p.grad = v  # gradient_as_bucket_view: the optimizer reads the averaged bucket in place
-            for v, g in self._shard_grads:
-                v.grad = g
+                        if id(p) not in unused:
+                            p.grad = v  # gradient_as_bucket_view: the optimizer reads the averaged bucket in place
+            for v, g, p in self._shard_grads:
+                if id(p) not in unused:
+                    v.grad = g
             self._shard_grads_live = bool(self._shard_grads)
             if self._step_in_backward is not None:
                 self._step_in_backward._stepped_in_backward = True
@@ -394,6 +498,9 @@ class DistributedDataParallel(nn.Module):
             self._next_bucket = 0
             for b in self.buckets:
                 b.pending, b.ready, b.launched = len(b.params), False, False
+            if self.find_unused_parameters:
+                self._locally_used = array.array("i", bytes(4 * len(self._params)))
+                self._unused, self._unused_ids = [], set()
 
     # ---- measurement hooks used by bench.py (CUDA events on the comm stream, around every bucket kernel) ----
     def start_profile(self) -> None:

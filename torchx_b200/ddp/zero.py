@@ -114,6 +114,11 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                             f"not {getattr(optimizer_class, '__name__', optimizer_class)}")
         if not isinstance(model, DistributedDataParallel):
             raise TypeError("ZeroRedundancyOptimizer shards a torchx_b200.ddp.DistributedDataParallel")
+        if overlap_with_ddp and model.find_unused_parameters:
+            raise ValueError(
+                "overlap_with_ddp=True cannot be combined with find_unused_parameters=True: each bucket's step runs inside "
+                "its reduce-scatter, before the ranks know which parameters none of them used, so such a parameter would be "
+                "stepped with a zero gradient instead of skipped")
         groups = _normalize_groups(model._params if params is None else params)
         _check_groups(groups, model._params)
         if overlap_with_ddp:
@@ -147,7 +152,7 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                 v = b.param_flat[lo:hi]
                 self._views[id(b.params[i])] = (v, lo, hi)
                 if not overlap_with_ddp:
-                    model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block]))
+                    model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block], b.params[i]))
         inner_groups = []
         for g, ps in zip(self.param_groups, self._full_groups):
             inner = {k: val for k, val in g.items() if k != "params"}
@@ -306,7 +311,7 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         """Clears the gradient shards and the model parameters' ``.grad``.  Required between a step and the next synced
         backward: the reduced gradients live only in the shards, which a synced backward overwrites (it raises instead)."""
         self.model._shard_grads_live = False
-        for v, g in self.model._shard_grads:
+        for v, g, _ in self.model._shard_grads:
             if set_to_none:
                 v.grad = None
             else:
@@ -327,7 +332,7 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             raise RuntimeError("overlap_with_ddp=True does not support clip_grad_norm_: the update has already happened "
                                "during backward, before a global norm could be known")
         dev = self.model.device
-        grads = [v.grad for v, _ in self.model._shard_grads if v.grad is not None]
+        grads = [v.grad for v, _, _ in self.model._shard_grads if v.grad is not None]
         sq = torch.zeros(1, dtype=torch.float32, device=dev)
         if grads:
             sq = torch.stack([g.float().square().sum() for g in grads]).sum().reshape(1)
@@ -358,16 +363,21 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         keys_of = {id(p): self._keys(g) if self._stepped else [] for g, ps in zip(self.param_groups, self._full_groups) for p in ps}
         tensor_keys = [k for k in ("exp_avg", "exp_avg_sq", "max_exp_avg_sq", "momentum_buffer")
                        if any(k in ks for ks in keys_of.values())]
-        # Adam's scalar `step`: one fp32 per parameter from every rank, taken from the lowest rank that holds a slice.  Read
-        # before any collective is issued, so that no host sync waits behind them.
+        # Adam's scalar `step`: one fp32 per parameter from every rank, taken from the lowest rank that holds a slice, and
+        # after them a 1 for each parameter whose slice here has state (one that never had a gradient, unused on every rank
+        # since the start, has none, as in the unsharded optimizer).  Read before any collective is issued, so that no host
+        # sync waits behind them.
         n = len(params)
-        own_steps = torch.zeros(n, dtype=torch.float32, device=dev)
+        own_steps = torch.zeros(2 * n, dtype=torch.float32, device=dev)
         for i, p in enumerate(params):
-            st = self.optim.state.get(self._views[id(p)][0], {}).get("step") if id(p) in self._views else None
-            if st is not None:
-                own_steps[i : i + 1].copy_(st.reshape(1), non_blocking=True)
-        steps = torch.zeros(W * n, dtype=torch.float32, device=dev)
-        steps[r * n : (r + 1) * n].copy_(own_steps)
+            st = self.optim.state.get(self._views[id(p)][0], {}) if id(p) in self._views else {}
+            if st.get("step") is not None:
+                own_steps[i : i + 1].copy_(st["step"].reshape(1), non_blocking=True)
+            if st:
+                own_steps[n + i] = 1.0
+        n2 = 2 * n
+        steps = torch.zeros(W * n2, dtype=torch.float32, device=dev)
+        steps[r * n2 : (r + 1) * n2].copy_(own_steps)
         full: Dict[str, Dict[int, torch.Tensor]] = {k: {} for k in tensor_keys}
         for k in tensor_keys:
             for b in self.model.buckets:
@@ -385,14 +395,15 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                     for p, o, numel in zip(b.params, b.spec.offsets, b.spec.numels):
                         full[k][id(p)] = _view_like(host[o : o + numel], p).clone()
                 del buf, own
-        _ordered(self.comm, lambda s: self.comm.allgather_(steps, steps[r * n : (r + 1) * n], stream=s))
+        _ordered(self.comm, lambda s: self.comm.allgather_(steps, steps[r * n2 : (r + 1) * n2], stream=s))
         if r != to:
             return
-        steps_h = steps.view(W, n).cpu()
+        steps_h = steps.view(W, n2).cpu()
+        has_state = steps_h[:, n:].amax(0) > 0
         state: Dict[int, Dict[str, Any]] = {}
         for i, p in enumerate(params):
             entry: Dict[str, Any] = {}
-            for k in keys_of[id(p)]:
+            for k in keys_of[id(p)] if has_state[i] else []:
                 if k == "step":
                     owner = next(q for q in range(W) if _owns(self._where[id(p)], q))
                     entry[k] = steps_h[owner, i].clone()
