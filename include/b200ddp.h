@@ -52,7 +52,7 @@ extern "C" {
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
                             b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats,
-                            b2_bn_backward_reduce and b2_reduce, which only add symbols: a binding that needs them
+                            b2_bn_backward_reduce, b2_reduce and b2_reduce_scatter_step_bf16, which only add symbols: a binding that needs them
                             fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -356,6 +356,21 @@ typedef struct b2_optim {
 
 int b2_reduce_scatter_step(b2_comm_t* comm, size_t block, const b2_segment_t* segments, int n_segments, int mode, float scale,
                            const b2_optim_t* opt, void* stream);
+
+/*
+ * The same fused step for a bf16 bucket whose parameters have fp32 master weights (the ZeRO-1 mini-DDP's
+ * master_weights=True with overlap_with_ddp): mode B2_BF16, and the step updates this rank's block of the masters, not
+ * of the bf16 parameters, which it then writes from them:
+ *      g[i] = float( round_bf16( sum_r bf16( scale * segment_r(rank*block + i) ) ) )   (b2_reduce_scatter_gather's bits, widened)
+ *      master[i], state[i] <- step(group of i, master[i], g[i], state[i])
+ *      param_bf16[i] <- bf16(master[i])   (round to nearest even, NaN -> 0x7FFF: ATen's conversion on the device)
+ * for every element i of a run with a group; pad elements are not touched.  `opt->param` points at this rank's `block`
+ * fp32 masters, `param_bf16` at this rank's block of the bucket's bf16 parameter buffer; the state and runs are those of
+ * b2_reduce_scatter_step.  B2_EINVAL, before anything is launched, for the checks of b2_reduce_scatter_step (the mode
+ * check aside) and a null or not 16-byte aligned `param_bf16`.  At W == 1 the gradient is the local pass's rounding, as for fp32 buckets.
+ */
+int b2_reduce_scatter_step_bf16(b2_comm_t* comm, size_t block, const b2_segment_t* segments, int n_segments, float scale,
+                                const b2_optim_t* opt, void* param_bf16, void* stream);
 
 /*
  * All-to-all, a bit-exact copy of bytes (any dtype): out[r] <- the recv_bytes[r] bytes rank r sends this rank, in[j] is what

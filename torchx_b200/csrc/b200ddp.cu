@@ -1288,6 +1288,30 @@ static int optim_table(const char* fn, const b2_optim_t* opt, size_t block, OptD
   return B2_OK;
 }
 
+// The launches of one fused step, fp32 bucket or bf16 bucket: at W == 1 the local pass's grid and rounding, else one
+// reduce-scatter step kernel per stage-sized piece of the block.
+extern "C++" template <int MODE>
+cudaError_t launch_step(b2_comm* c, Src& src, typename OptOf<MODE>::type& o, size_t block, float scale, void* stream) {
+  const int W = c->d.world;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (W == 1) {
+    k_local_step<MODE><<<local_grid(block, sm_count(c->device)), kThreads, 0, s>>>(src, o, block, scale);
+    c->launches++;
+    return cudaGetLastError();
+  }
+  const size_t cap = c->d.slice_cap / dev::Wire<MODE>::kBytes * 8;  // elements of a block one recv region holds
+  return for_chunks(c, block, cap, [&](size_t off, size_t n) {
+    src.off = off;  // the same block offset for the gradient table and the parameter / state slices
+    o.off = off;
+    cudaError_t le = cudaErrorInvalidValue;
+    with_world(W, [&](auto w) {
+      k_reduce_scatter_step<MODE, decltype(w)::value><<<grid_for(c, (n + 7) / 8, 1), kThreads, 0, s>>>(c->d, src, o, n, block, scale);
+      le = cudaGetLastError();
+    });
+    return le;
+  });
+}
+
 int b2_reduce_scatter_step(b2_comm_t* c, size_t block, const b2_segment_t* segments, int n_segments, int mode, float scale,
                            const b2_optim_t* opt, void* stream) {
   if (mode != B2_F32_WIRE_BF16 && mode != B2_F32 && mode != B2_F32_WIRE_F16)
@@ -1301,30 +1325,31 @@ int b2_reduce_scatter_step(b2_comm_t* c, size_t block, const b2_segment_t* segme
   if (const int rc = segment_table("b2_reduce_scatter_step", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
   cudaError_t e = cudaErrorInvalidValue;
   with_mode(mode, [&](auto m) {
     constexpr int MODE = decltype(m)::value;
-    if constexpr (!k16BitBucket<MODE>) {
-      if (W == 1) {  // the local pass's grid and rounding
-        k_local_step<MODE><<<local_grid(block, sm_count(c->device)), kThreads, 0, s>>>(src, o, block, scale);
-        c->launches++;
-        e = cudaGetLastError();
-        return;
-      }
-      const size_t cap = c->d.slice_cap / dev::Wire<MODE>::kBytes * 8;  // elements of a block one recv region holds
-      e = for_chunks(c, block, cap, [&](size_t off, size_t n) {
-        src.off = off;  // the same block offset for the gradient table and the parameter / state slices
-        o.off = off;
-        cudaError_t le = cudaErrorInvalidValue;
-        with_world(W, [&](auto w) {
-          k_reduce_scatter_step<MODE, decltype(w)::value><<<grid_for(c, (n + 7) / 8, 1), kThreads, 0, s>>>(c->d, src, o, n, block, scale);
-          le = cudaGetLastError();
-        });
-        return le;
-      });
-    }
+    if constexpr (!k16BitBucket<MODE>) e = launch_step<MODE>(c, src, o, block, scale, stream);
   });
+  if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter step kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+int b2_reduce_scatter_step_bf16(b2_comm_t* c, size_t block, const b2_segment_t* segments, int n_segments, float scale,
+                                const b2_optim_t* opt, void* param_bf16, void* stream) {
+  if (block == 0) return B2_OK;
+  OptDevBf16 o;  // checked first: it needs no communicator
+  if (const int rc = optim_table("b2_reduce_scatter_step_bf16", opt, block, o)) return rc;
+  if (!param_bf16) return fail(B2_EINVAL, "b2_reduce_scatter_step_bf16: null bf16 parameter pointer");
+  if (reinterpret_cast<uintptr_t>(param_bf16) & 15u)
+    return fail(B2_EINVAL, "b2_reduce_scatter_step_bf16: bf16 parameter pointer not 16-byte aligned");
+  o.pbf = static_cast<uint16_t*>(param_bf16);
+  if (!c) return fail(B2_EINVAL, "null communicator");
+  const int W = c->d.world;
+  Src src;
+  if (const int rc = segment_table("b2_reduce_scatter_step_bf16", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
+  if (const int rc = check_not_poisoned(c)) return rc;
+  DeviceGuard g(c->device);
+  const cudaError_t e = launch_step<B2_BF16>(c, src, o, block, scale, stream);
   if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter step kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }

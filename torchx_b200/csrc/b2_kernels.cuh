@@ -42,8 +42,9 @@ __global__ void __launch_bounds__(kThreads) k_local_pass(const __grid_constant__
 // W == 1 with the optimizer step (b2_reduce_scatter_step): the local pass's rounding of each vec read through the segment
 // table (mode 0 is not a copy: it rounds to bf16), then the optimizer epilogue on the parameter and state slices
 // (b2_optim.cuh) instead of the store.  The local pass's CTA layout, so a thread's segment and run hints keep hitting.
+// MODE B2_BF16 is b2_reduce_scatter_step_bf16's: fp32 masters stepped, bf16 parameters written.
 template <int MODE>
-__global__ void __launch_bounds__(kThreads, 1) k_local_step(const __grid_constant__ Src src, const __grid_constant__ OptDev o,
+__global__ void __launch_bounds__(kThreads, 1) k_local_step(const __grid_constant__ Src src, const __grid_constant__ typename OptOf<MODE>::type o,
                                                          unsigned long long n, float scale) {
   using namespace dev;
   __shared__ OptCta t;

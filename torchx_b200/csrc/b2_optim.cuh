@@ -43,6 +43,22 @@ struct OptDev {
   OptGroupDev g[kOptMaxGroups];
 };
 
+// The bf16 bucket's step (b2_reduce_scatter_step_bf16): `param` is this rank's block of fp32 master weights, and every
+// element the step updates is also written, converted to bf16, to the same block of the bucket's bf16 parameters.
+struct OptDevBf16 : OptDev {
+  uint16_t* pbf;  // element 0 of this rank's block of the bf16 parameter buffer
+};
+
+// The table a mode's step kernels take: fp32 buckets step their parameters in place, a bf16 bucket steps masters.
+template <int MODE>
+struct OptOf {
+  using type = OptDev;
+};
+template <>
+struct OptOf<B2_BF16> {
+  using type = OptDevBf16;
+};
+
 }  // namespace
 
 namespace dev {
@@ -116,6 +132,21 @@ __device__ __forceinline__ void opt_elem(const OptDev& o, const OptCta& t, int k
   p = __fsub_rn(p, __fdiv_rn(__fmul_rn(t.step_size[k], m), denom));  // p -= step_size * m / denom
 }
 
+// The bf16 mirror of the stepped masters: no-ops for an fp32 bucket's table, stores for a bf16 bucket's.  The conversion
+// is the one ATen's CUDA kernels make on sm_80 and later (c10::BFloat16 from float is __float2bfloat16 there, one
+// cvt.rn.bf16.f32): round to nearest even, and every NaN becomes the canonical 0x7FFF.  So the bf16 parameters get the
+// bits of `param.copy_(master)` on the device.  `pbf` is 16-byte aligned (checked on the host) and a vec starts at a block
+// element that is a multiple of 8, so the vector path's 16-byte store is aligned whenever its fp32 accesses are.
+__device__ __forceinline__ void mirror_vec(const OptDev&, unsigned long long, const F8&) {}
+__device__ __forceinline__ void mirror_elem(const OptDev&, unsigned long long, float) {}
+__device__ __forceinline__ void mirror_vec(const OptDevBf16& o, unsigned long long b, const F8& p) {
+  stg_u4(o.pbf + b, make_uint4(pack_bf16x2(p.v[0], p.v[1]), pack_bf16x2(p.v[2], p.v[3]), pack_bf16x2(p.v[4], p.v[5]),
+                                pack_bf16x2(p.v[6], p.v[7])));
+}
+__device__ __forceinline__ void mirror_elem(const OptDevBf16& o, unsigned long long b, float p) {
+  o.pbf[b] = static_cast<uint16_t>(pack_bf16x2(p, 0.f) & 0xffffu);
+}
+
 // The run a thread looked at last: successive vecs of one thread usually stay inside one parameter.
 struct RunHint {
   int k = 0;
@@ -138,8 +169,10 @@ __device__ __forceinline__ int opt_run(const OptDev& o, RunHint& h, unsigned lon
 }
 
 // The epilogue on one vec: launch elements [e, e + 8) of n, reduced gradient `gr` (fp32 values).  Loads this rank's
-// parameter and state slices at the same block offset, steps the elements that belong to a group, stores them back.
-__device__ __forceinline__ void opt_step_vec(const OptDev& o, const OptCta& t, RunHint& h, unsigned long long e, unsigned long long n,
+// parameter and state slices at the same block offset, steps the elements that belong to a group, stores them back (and,
+// with a bf16 bucket's table, their bf16 conversions into the bf16 parameters).
+template <class O>
+__device__ __forceinline__ void opt_step_vec(const O& o, const OptCta& t, RunHint& h, unsigned long long e, unsigned long long n,
                                              const F8& gr) {
   const unsigned long long b = o.off + e;  // block coordinates
   const int k0 = opt_run(o, h, b);
@@ -159,6 +192,7 @@ __device__ __forceinline__ void opt_step_vec(const OptDev& o, const OptCta& t, R
 #pragma unroll
     for (int i = 0; i < 8; ++i) opt_elem(o, t, k0, b + i, p.v[i], gr.v[i], m.v[i], v.v[i]);
     stg_f8(pp, p);
+    mirror_vec(o, b, p);
     if (mom) stg_f8(p0, m);
     if (adam) stg_f8(p1, v);
     return;
@@ -175,6 +209,7 @@ __device__ __forceinline__ void opt_step_vec(const OptDev& o, const OptCta& t, R
     float p = pp[i], m = mom ? p0[i] : 0.f, v = adam ? p1[i] : 0.f;
     opt_elem(o, t, k, b + i, p, gr.v[i], m, v);
     pp[i] = p;
+    mirror_elem(o, b + i, p);
     if (mom) p0[i] = m;
     if (adam) p1[i] = v;
   }

@@ -99,10 +99,12 @@ __global__ void __launch_bounds__(kThreads, 1)
 
 // The same reduce-scatter with the optimizer step as its phase B epilogue (b2_reduce_scatter_step, b2_optim.cuh): the
 // reduced vec is rounded as `out` would hold it, then steps this rank's parameter and state slices at the same block
-// offset.  Phase B runs one vec per trip: the epilogue's three loads and stores per element need the registers.
+// offset.  Phase B runs one vec per trip: the epilogue's three loads and stores per element need the registers.  The bf16
+// bucket's instances (b2_reduce_scatter_step_bf16) step fp32 masters with the bf16-rounded gradient and write the bf16
+// parameters next to them.
 template <int MODE, int W>
 __global__ void __launch_bounds__(kThreads, 1)
-    k_reduce_scatter_step(CommDev c, const __grid_constant__ Src src, const __grid_constant__ OptDev o, unsigned long long n,
+    k_reduce_scatter_step(CommDev c, const __grid_constant__ Src src, const __grid_constant__ typename OptOf<MODE>::type o, unsigned long long n,
                           unsigned long long block, float scale) {
   using namespace dev;
   constexpr int WVB = Wire<MODE>::kBytes;

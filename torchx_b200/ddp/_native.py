@@ -144,6 +144,7 @@ SIGNATURES = {
     "b2_reduce": (_i, [_vp, _vp, _sz, _i, _i, _i, _vp]),
     "b2_reduce_scatter_gather": (_i, [_vp, _vp, _sz, _P(B2Segment), _i, _i, _f, _vp]),
     "b2_reduce_scatter_step": (_i, [_vp, _sz, _P(B2Segment), _i, _i, _f, _P(B2Optim), _vp]),
+    "b2_reduce_scatter_step_bf16": (_i, [_vp, _sz, _P(B2Segment), _i, _f, _P(B2Optim), _vp, _vp]),
     "b2_alltoall": (_i, [_vp, _P(_vp), _P(_sz), _P(_vp), _P(_sz), _vp]),
     "b2_alltoall_max_bytes": (_sz, [_vp]),
     "b2_p2p": (_i, [_vp, _P(B2P2pOp), _i, _vp]),

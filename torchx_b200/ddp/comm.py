@@ -306,6 +306,18 @@ class Communicator:
         N.check(N.lib().b2_reduce_scatter_step(self._h, block, segments, n_segments, mode, self._scale(scale),
                                                ctypes.byref(opt), _stream_arg(stream, self.device)))
 
+    def reduce_scatter_step_bf16_(self, block: int, segments, n_segments: int, opt, param_bf16: torch.Tensor,
+                                  scale: Optional[float] = None, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """``reduce_scatter_step_`` for a bf16 bucket with fp32 master weights (include/b200ddp.h:
+        b2_reduce_scatter_step_bf16): ``opt.param`` is this rank's block of fp32 masters, which the step updates with the
+        bf16 reduced gradient; ``param_bf16`` (this rank's ``block`` elements of the bucket's bf16 parameter buffer) is
+        written from every stepped master.  The overlap mode of the sharded mini-DDP with ``master_weights=True``."""
+        self._check_tensor(param_bf16)
+        if param_bf16.dtype != torch.bfloat16 or param_bf16.numel() != block or not param_bf16.is_contiguous():
+            raise ValueError(f"param_bf16 must be {block} contiguous bf16 elements, got {param_bf16.numel()} of {param_bf16.dtype}")
+        N.check(N.lib().b2_reduce_scatter_step_bf16(self._h, block, segments, n_segments, self._scale(scale), ctypes.byref(opt),
+                                                    ctypes.c_void_p(param_bf16.data_ptr()), _stream_arg(stream, self.device)))
+
     def alltoall_(self, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor],
                   stream: Optional[torch.cuda.Stream] = None) -> Sequence[torch.Tensor]:
         """``outs[r]`` <- the ``ins[rank]`` of rank r, bit for bit (include/b200ddp.h: b2_alltoall).  Both are lists of world

@@ -147,6 +147,7 @@ class _Bucket:
 
 class DistributedDataParallel(nn.Module):
     find_unused_parameters = False  # the constructor's keyword; a class default, so an instance built without __init__ has it
+    _shard_widen = ()  # ZeRO-1 master weights without overlap: (bf16 gradient shard, fp32 block) widened after each backward
 
     def __init__(
         self,
@@ -449,7 +450,11 @@ class DistributedDataParallel(nn.Module):
             t0 = torch.cuda.Event(enable_timing=True)
             t0.record(self._comm_stream)
         # the gradients (and the scratch copy) stay referenced until _finalize_backward has made the compute stream wait
-        if zero is not None:  # hyper-parameters read now: a scheduler stepped after step() reaches the next backward
+        if zero is not None and zero.master_weights and b.dtype == torch.bfloat16:  # steps the masters, writes the bf16 block
+            self.comm.reduce_scatter_step_bf16_(b.block, segs, len(segs), zero._launch_table(b),
+                                                b.param_flat[self.comm.rank * b.block : (self.comm.rank + 1) * b.block],
+                                                scale=1.0 / self.world_size, stream=self._comm_stream)
+        elif zero is not None:  # hyper-parameters read now: a scheduler stepped after step() reaches the next backward
             self.comm.reduce_scatter_step_(b.block, segs, len(segs), zero._launch_table(b), scale=1.0 / self.world_size,
                                            wire=self.wire, stream=self._comm_stream)
         else:
@@ -486,6 +491,8 @@ class DistributedDataParallel(nn.Module):
                     for p, v in zip(b.params, b.views):
                         if id(p) not in unused:
                             p.grad = v  # gradient_as_bucket_view: the optimizer reads the averaged bucket in place
+            for src, dst in self._shard_widen:  # the fp32 gradients the inner optimizer steps the masters with
+                dst.copy_(src)
             for v, g, p in self._shard_grads:
                 if id(p) not in unused:
                     v.grad = g

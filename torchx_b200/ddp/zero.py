@@ -11,6 +11,10 @@ This one runs on the native communicator instead:
 SGD, Adam and AdamW are elementwise, so stepping a slice gives the bits of stepping the whole tensor, with two exceptions
 in torch's fused kernels (DESIGN.md 2.4) that the constructor refuses where they would apply: the parameters stay
 bit-equal to those of the unsharded mini-DDP under the same optimizer, and the consolidated state to its state.
+
+With ``master_weights=True`` a bf16 model trains on fp32 master weights, each rank holding only its block of them: the
+inner optimizer steps the masters with the widened bf16 gradient shard, and this rank's block of the bf16 parameters is
+written from them (ATen's fp32 -> bf16 conversion) before the all-gather (DESIGN.md 2.5).
 """
 from __future__ import annotations
 
@@ -103,12 +107,20 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
 
     After a synced backward the model parameters' ``.grad`` are None (the reduced gradients exist only as the shards), so
     clip with ``clip_grad_norm_`` of this class: ``torch.nn.utils.clip_grad_norm_(model.parameters(), ...)`` sees no
-    gradients and clips nothing."""
+    gradients and clips nothing.
+
+    ``master_weights=True`` keeps fp32 master weights for the model's bf16 parameters, sharded like the state: the inner
+    optimizer, ``param_groups``, ``state`` and schedulers work on 1-D fp32 views of this rank's masters, and every step
+    writes the bf16 parameters from them.  fp32 parameters of the same model are stepped as without the flag; fp16 ones
+    are refused (they would need loss scaling on the masters), and so is GradScaler.  The masters are taken from the bf16
+    parameters at construction: load the module's weights before constructing the optimizer, or restore the masters
+    with ``load_state_dict`` (its ``"master_params"``), or the next step overwrites the loaded weights from stale
+    masters."""
 
     _step_supports_amp_scaling = True  # GradScaler hands itself to step(): the found-inf decision is made rank-global there
 
     def __init__(self, model: DistributedDataParallel, optimizer_class: type, params: Optional[Any] = None,
-                 overlap_with_ddp: bool = False, **defaults: Any) -> None:
+                 overlap_with_ddp: bool = False, master_weights: bool = False, **defaults: Any) -> None:
         if optimizer_class not in SUPPORTED:
             raise TypeError(f"ZeroRedundancyOptimizer supports {', '.join(c.__name__ for c in SUPPORTED)}, "
                             f"not {getattr(optimizer_class, '__name__', optimizer_class)}")
@@ -121,9 +133,11 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                 "stepped with a zero gradient instead of skipped")
         groups = _normalize_groups(model._params if params is None else params)
         _check_groups(groups, model._params)
+        if master_weights:
+            _check_masters(model._params)
         if overlap_with_ddp:
             model._check_shardable()
-            _check_overlap(groups, defaults, model)
+            _check_overlap(groups, defaults, model, master_weights)
             gi_of = {id(p): gi for gi, g in enumerate(groups) for p in g["params"]}
             pos = [optimizer_class is torch.optim.Adam and bool({**defaults, **g}.get("weight_decay", 0)) for g in groups]
             _check_run_bound([[gi_of[id(p)] for p in b.params] for b in model.buckets],
@@ -136,6 +150,7 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         self.comm = model.comm
         self.optimizer_class = optimizer_class
         self.overlap_with_ddp = overlap_with_ddp
+        self.master_weights = master_weights
         self._full_groups = [list(g["params"]) for g in self.param_groups]  # model parameters, the user's order
         model._enable_sharding(self if overlap_with_ddp else None)
 
@@ -145,14 +160,29 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             for p, o, n in zip(b.params, b.spec.offsets, b.spec.numels):
                 where[id(p)] = (b, o, n)
         self._where = where
-        # views[id(param)] = (view of the flat parameter buffer, bucket elements lo, hi): this rank's slice of it
+        # master_weights: bucket index -> this rank's block of fp32 masters of a bf16 bucket (the exact widening of its bf16
+        # parameters), and without overlap the fp32 gradient block the inner optimizer reads (the widened gradient shard,
+        # written after every synced backward)
+        self._master_flat: Dict[int, torch.Tensor] = {}
+        self._master_grad: Dict[int, torch.Tensor] = {}
+        for bi, b in enumerate(model.buckets):
+            if master_weights and b.dtype == torch.bfloat16:
+                self._master_flat[bi] = b.param_flat[r * b.block : (r + 1) * b.block].float()
+                if not overlap_with_ddp:
+                    self._master_grad[bi] = torch.zeros(b.block, dtype=torch.float32, device=model.device)
+        if self._master_grad:
+            model._shard_widen = [(model.buckets[bi].shard_grad, g) for bi, g in self._master_grad.items()]
+        # views[id(param)] = (the inner optimizer's view, bucket elements lo, hi): this rank's slice of the flat parameter
+        # buffer, or of the masters for a parameter that has them
         self._views: Dict[int, Tuple[torch.Tensor, int, int]] = {}
-        for b in model.buckets:
+        for bi, b in enumerate(model.buckets):
+            m = self._master_flat.get(bi)
             for i, lo, hi in block_intersections(b.spec.offsets, b.spec.numels, b.block, r):
-                v = b.param_flat[lo:hi]
+                a, z = lo - r * b.block, hi - r * b.block
+                v = b.param_flat[lo:hi] if m is None else m[a:z]
                 self._views[id(b.params[i])] = (v, lo, hi)
                 if not overlap_with_ddp:
-                    model._shard_grads.append((v, b.shard_grad[lo - r * b.block : hi - r * b.block], b.params[i]))
+                    model._shard_grads.append((v, (b.shard_grad if m is None else self._master_grad[bi])[a:z], b.params[i]))
         inner_groups = []
         for g, ps in zip(self.param_groups, self._full_groups):
             inner = {k: val for k, val in g.items() if k != "params"}
@@ -214,13 +244,13 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                 self.optim.state[v] = st
 
     def _launch_table(self, b) -> "N.B2Optim":
-        """The b2_optim_t of one bucket launch: this rank's parameter and state blocks, its runs (adjacent parameters of
+        """The b2_optim_t of one bucket launch: this rank's parameter (or master) and state blocks, its runs (adjacent parameters of
         one group and step count coalesced) and every group's hyper-parameters as param_groups hold them now."""
         bi = self._bucket_index[id(b)]
         t = N.B2Optim()
         t.kind = self._kind
         t.n_groups = len(self.param_groups)
-        t.param = b.param_flat[self._rank * b.block :].data_ptr()
+        t.param = self._master_flat[bi].data_ptr() if bi in self._master_flat else b.param_flat[self._rank * b.block :].data_ptr()
         flat = self._flat_state[bi]
         t.state0 = flat[self._state_keys[0]].data_ptr()
         t.state1 = flat["exp_avg_sq"].data_ptr() if "exp_avg_sq" in flat else None
@@ -259,6 +289,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         apart.  Should torch drop the keyword, ``step()`` stops being called with it and a GradScaler run raises below."""
         if closure is not None:
             raise RuntimeError("ZeroRedundancyOptimizer.step does not take a closure")
+        if self.master_weights and (grad_scaler is not None or getattr(self, "found_inf", None) is not None):
+            raise RuntimeError("master_weights=True does not support GradScaler: bf16 parameters need no loss scaling")
         if self.overlap_with_ddp:
             return self._step_overlap(grad_scaler)
         if grad_scaler is None and getattr(self, "found_inf", None) is not None:
@@ -278,6 +310,9 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                 return None
         self.optim.step()
         self._stepped = True
+        for bi, m in self._master_flat.items():  # this rank's bf16 parameters from the stepped masters
+            b = self.model.buckets[bi]
+            b.param_flat[self._rank * b.block : (self._rank + 1) * b.block].copy_(m)
         for b in self.model.buckets:
             own = b.param_flat[self._rank * b.block : (self._rank + 1) * b.block]
             _ordered(self.comm, lambda s, b=b, own=own: self.comm.allgather_(b.param_flat, own, stream=s))
@@ -327,7 +362,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
     def clip_grad_norm_(self, max_norm: float) -> torch.Tensor:
         """Clips the sharded gradients in place by their global 2-norm and returns that norm (fp32, the same bits on
         every rank): the sqrt of the rank-order fp32 sum of each rank's fp32 sum of squares over its shard.  The clip
-        coefficient is torch's, ``max_norm / (norm + 1e-6)`` clamped to 1."""
+        coefficient is torch's, ``max_norm / (norm + 1e-6)`` clamped to 1.  With master weights the gradients clipped
+        are the masters' fp32 ones."""
         if self.overlap_with_ddp:
             raise RuntimeError("overlap_with_ddp=True does not support clip_grad_norm_: the update has already happened "
                                "during backward, before a global norm could be known")
@@ -380,8 +416,8 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         steps[r * n2 : (r + 1) * n2].copy_(own_steps)
         full: Dict[str, Dict[int, torch.Tensor]] = {k: {} for k in tensor_keys}
         for k in tensor_keys:
-            for b in self.model.buckets:
-                buf = torch.zeros(W * b.block, dtype=b.dtype, device=dev)
+            for bi, b in enumerate(self.model.buckets):
+                buf = torch.zeros(W * b.block, dtype=torch.float32 if bi in self._master_flat else b.dtype, device=dev)
                 for p in b.params:
                     if id(p) in self._views:
                         v, lo, hi = self._views[id(p)]
@@ -395,6 +431,18 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                     for p, o, numel in zip(b.params, b.spec.offsets, b.spec.numels):
                         full[k][id(p)] = _view_like(host[o : o + numel], p).clone()
                 del buf, own
+        masters: Dict[int, torch.Tensor] = {}  # id(param) -> its full fp32 master, gathered like the state
+        for bi, m in self._master_flat.items():
+            b = self.model.buckets[bi]
+            buf = torch.zeros(W * b.block, dtype=torch.float32, device=dev)
+            own = buf[r * b.block : (r + 1) * b.block]
+            own.copy_(m)
+            _ordered(self.comm, lambda s, buf=buf, own=own: self.comm.allgather_(buf, own, stream=s))
+            if r == to:
+                host = buf.cpu()
+                for p, o, numel in zip(b.params, b.spec.offsets, b.spec.numels):
+                    masters[id(p)] = _view_like(host[o : o + numel], p).clone()
+            del buf, own
         _ordered(self.comm, lambda s: self.comm.allgather_(steps, steps[r * n2 : (r + 1) * n2], stream=s))
         if r != to:
             return
@@ -418,20 +466,29 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             at += len(ps)
             groups.append(d)
         self._consolidated = {"state": state, "param_groups": groups}
+        if self.master_weights:  # the full fp32 masters in param index order, None for a parameter without one
+            self._consolidated["master_params"] = [masters.get(id(p)) for p in params]
 
     def state_dict(self) -> Dict[str, Any]:
         """After ``consolidate_state_dict(to)``, on rank ``to``: the state dict of the unsharded optimizer (its
-        param_groups and param indices; full-size per-parameter state)."""
+        param_groups and param indices; full-size per-parameter state).  With master weights the state is that of an
+        optimizer over the fp32 masters, and ``"master_params"`` lists the full masters in param index order (None for an
+        fp32 parameter)."""
         sd = getattr(self, "_consolidated", None)
         if sd is None:
             raise RuntimeError("call consolidate_state_dict(to) on every rank first; state_dict() returns on rank `to` only")
         return sd
 
     def load_state_dict(self, state_dict: Dict[str, Any]) -> None:
-        """Loads the full (unsharded) form on every rank, keeping this rank's slices."""
+        """Loads the full (unsharded) form on every rank, keeping this rank's slices.  With master weights, this rank's
+        slices of ``"master_params"`` become the masters; a state dict without that key re-derives them from the current
+        bf16 parameters."""
         groups = state_dict["param_groups"]
         if len(groups) != len(self._full_groups) or any(len(g["params"]) != len(ps) for g, ps in zip(groups, self._full_groups)):
             raise ValueError("the state dict's param groups do not match this optimizer's")
+        masters = state_dict.get("master_params") if self.master_weights else None
+        if masters is not None and len(masters) != len(self._index()):
+            raise ValueError(f"the state dict has {len(masters)} master_params, this optimizer {len(self._index())} parameters")
         if self.overlap_with_ddp:
             self._check_loaded_runs(state_dict)
         inner_state: Dict[int, Dict[str, Any]] = {}
@@ -460,8 +517,28 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         self._stepped = bool(state_dict["state"])
         self.param_groups = self.optim.param_groups
         self.state = self.optim.state
+        if self.master_weights:
+            self._load_masters(masters)
         if self.overlap_with_ddp:
             self._land_loaded_state()
+
+    @torch.no_grad()
+    def _load_masters(self, masters: Optional[List[Optional[torch.Tensor]]]) -> None:
+        """This rank's master blocks from the full masters in param index order, or (None) from the bf16 parameters."""
+        r = self._rank
+        index = {id(p): i for i, p in enumerate(self._index())}
+        for bi, m in self._master_flat.items():
+            b = self.model.buckets[bi]
+            if masters is None:
+                m.copy_(b.param_flat[r * b.block : (r + 1) * b.block])
+                continue
+            for p, o in zip(b.params, b.spec.offsets):
+                if id(p) not in self._views:
+                    continue
+                _, lo, hi = self._views[id(p)]
+                mem = _view_like(torch.empty(p.numel(), dtype=torch.float32, device=p.device), p)
+                mem.copy_(masters[index[id(p)]])  # the parameter's memory order, as the flat buffer holds it
+                m[lo - r * b.block : hi - r * b.block].copy_(mem.as_strided((p.numel(),), (1,))[lo - o : hi - o])
 
     def _check_loaded_runs(self, state_dict: Dict[str, Any]) -> None:
         """Overlap mode, before loading: the run bound with the checkpoint's step counts (the same on every rank)."""
@@ -502,11 +579,23 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
         self._attach_state()
 
 
-def _check_overlap(groups: List[Dict[str, Any]], defaults: Dict[str, Any], model: DistributedDataParallel) -> None:
+def _check_masters(params: Sequence[torch.nn.Parameter]) -> None:
+    """master_weights=True: fp32 masters for bf16 parameters; fp32 ones are stepped as they are."""
+    if any(p.dtype == torch.float16 for p in params):
+        raise TypeError("master_weights=True keeps fp32 masters for bf16 parameters only: fp16 parameters would need loss "
+                        "scaling on the masters")
+    if not any(p.dtype == torch.bfloat16 for p in params):
+        raise ValueError("master_weights=True needs bf16 parameters: the model has none (fp32 parameters are their own "
+                         "masters)")
+
+
+def _check_overlap(groups: List[Dict[str, Any]], defaults: Dict[str, Any], model: DistributedDataParallel,
+                   master_weights: bool = False) -> None:
     """What the fused step inside the reduce-scatter cannot do, refused before anything is sharded."""
     if model.wire not in ("bf16", "f32", "f16"):
         raise ValueError(f"overlap_with_ddp=True: unknown wire format {model.wire!r}")
-    if any(p.dtype != torch.float32 for p in model._params):
+    stepped = (torch.float32, torch.bfloat16) if master_weights else (torch.float32,)  # bf16: through its fp32 masters
+    if any(p.dtype not in stepped for p in model._params):
         raise TypeError("overlap_with_ddp=True steps fp32 parameters only (modes B2_F32_WIRE_BF16, B2_F32, B2_F32_WIRE_F16)")
     if len(groups) > N.B2_OPT_MAX_GROUPS:
         raise ValueError(f"overlap_with_ddp=True takes at most {N.B2_OPT_MAX_GROUPS} parameter groups, got {len(groups)}")
