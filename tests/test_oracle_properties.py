@@ -62,9 +62,22 @@ def test_two_ranks_commute_and_negation_is_exact(xs, scale):
     if len(xs) == 2:
         for mode in MODES:
             assert_bits_equal(oracle.allreduce(mode, xs, scale), oracle.allreduce(mode, xs[::-1], scale), "a+b == b+a")
-    for mode in MODES:  # round-to-nearest-even is symmetric
+    for mode in MODES:  # round-to-nearest-even is symmetric, except for the sign of an exact cancellation (below)
         pos, neg = oracle.allreduce(mode, xs, scale), oracle.allreduce(mode, [-x for x in xs], scale)
-        assert_bits_equal(neg, -pos, "negation")
+        zero = (pos == 0) & (neg == 0)  # c + (-c) is +0 whatever c's sign: both sides may hold +0
+        assert_bits_equal(np.where(zero, np.float32(0), neg), np.where(zero, np.float32(0), -pos), "negation")
+
+
+def test_exact_cancellation_is_positive_zero_on_both_sides():
+    """IEEE 754 round-to-nearest: a sum that cancels exactly is +0, and a sum of zeros is -0 only when every zero is -0."""
+    a = np.array([1.5, 0.0, -0.0, -0.0, 3e-39], np.float32)
+    b = np.array([-1.5, -0.0, 0.0, -0.0, -3e-39], np.float32)
+    for mode in MODES:
+        for scale in (1.0, 0.5):
+            for xs, want in (([a, b], [0, 0, 0, 0x80000000, 0]), ([-a, -b], [0, 0, 0, 0, 0])):
+                got = oracle.allreduce(mode, xs, scale)
+                assert got.view(np.uint32).tolist() == want, (mode, scale, got.view(np.uint32).tolist())
+                assert_bits_equal(got, allreduce_numpy(mode, xs, scale), "numpy twin")
 
 
 @settings(**SETTINGS)

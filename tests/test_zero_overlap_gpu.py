@@ -1,14 +1,15 @@
 """b2_reduce_scatter_step and ZeroRedundancyOptimizer(overlap_with_ddp=True) on the GPU, all ranks sharing one device.
 
-Kernel: the fused step against reduce_scatter_gather_ into a shard followed by torch._fused_sgd_ / _fused_adam_ /
-_fused_adamw_ on the same slices with the same hyper-parameters, parameters and state bit for bit, the pad untouched.
+Kernel: the fused step against torch._fused_sgd_ / _fused_adam_ / _fused_adamw_ on the oracle's block of the reduced
+gradients (which reduce_scatter_gather_ into a shard must equal too), same slices, same hyper-parameters, parameters and
+state bit for bit, the pad untouched.
 Mini-DDP: overlap mode against the unsharded mini-DDP with the same optimizer class and fused=True, bit for bit after
 every step and in the consolidated state; no_sync, checkpoints, the copy-in fallback and the run-time errors."""
 import numpy as np
 import pytest
 import torch
 
-from tests.test_zero_gpu import (WIRE, _assert_same, _assert_state_equal, _consolidate, _ddps, _input, _params, _phase,
+from tests.test_zero_gpu import (WIRE, _assert_same, _assert_state_equal, _consolidate, _ddps, _input, _oracle, _params, _phase,
                                  _pieces, _warm, _world)
 from torchx_b200.ddp import _native as N
 from torchx_b200.ddp import zero as Z
@@ -88,9 +89,11 @@ def _check(W, mode, n, kind, seed, n_steps=3, stage_mb=8, adam_step0=0, aligned=
     groups = [i % 2 for i in range(len(sizes))]  # neighbours in different groups, so groups meet inside vecs
     hyper = HYPER[kind]
     wire = WIRE[mode]
-    tables, keep = [], []
+    tables, keep, xs = [], [], []
     for r in range(W):
-        x = torch.randn(n, generator=torch.Generator().manual_seed(seed * 10 + r)).cuda()
+        x = torch.randn(n, generator=torch.Generator().manual_seed(seed * 10 + r))
+        xs.append(np.concatenate([x.numpy(), np.zeros(W * B - n, np.float32)]))
+        x = x.cuda()
         segs = (N.B2Segment * (len(sizes) + 1))()
         for i, (o, k) in enumerate(zip(offsets, sizes)):
             off = 0 if aligned else i % 2
@@ -112,6 +115,10 @@ def _check(W, mode, n, kind, seed, n_steps=3, stage_mb=8, adam_step0=0, aligned=
     ref = [(p.clone(), m.clone(), v.clone()) for p, m, v in zip(P, M, V)]
     runs = [Z.block_runs(offsets, sizes, groups, B, r) for r in range(W)]
     shards = [torch.empty(B, device="cuda") for _ in range(W)]
+    # the reference steps the oracle's block, not the library's reduce-scatter: a reduction that both kernels got wrong
+    # alike (a summation order, say) must not cancel out
+    reduced = _oracle(mode, xs, 1.0 / W)
+    blocks = [torch.from_numpy(reduced[r * B:(r + 1) * B].copy()).cuda() for r in range(W)]
     torch.cuda.synchronize()
     for step in range(adam_step0, adam_step0 + n_steps):
         counts = [[None if i is None else step for *_, i in rs] for rs in runs]
@@ -125,13 +132,14 @@ def _check(W, mode, n, kind, seed, n_steps=3, stage_mb=8, adam_step0=0, aligned=
         w.run(lambda r, c, s: c.reduce_scatter_gather_(shards[r], tables[r][0], tables[r][1], scale=1.0 / W, wire=wire,
                                                        stream=s))
         for r in range(W):
-            _reference(kind, hyper, shards[r], *ref[r], runs[r], [step] * len(runs[r]))
+            _reference(kind, hyper, blocks[r], *ref[r], runs[r], [step] * len(runs[r]))
         torch.cuda.synchronize()
         what = f"W={W} mode={mode} n={n} {kind} step {step}"
         for r in range(W):
             for name, got, want in zip("pmv", (P[r], M[r], V[r]), ref[r]):
                 assert torch.equal(got.view(torch.int32), want.view(torch.int32)), (
                     f"{what} rank {r} {name}: {(got != want).nonzero()[:8].flatten().tolist()}")
+            assert torch.equal(shards[r].view(torch.int32), blocks[r].view(torch.int32)), f"{what} rank {r}: shard vs oracle"
 
 
 @pytest.mark.parametrize("kind", ["sgd", "sgd0", "adam", "adamw"])
