@@ -290,6 +290,7 @@ class DistributedDataParallel(nn.Module):
     def forward(self, *args, **kwargs):
         synced = torch.is_grad_enabled() and self.require_backward_grad_sync
         if synced:
+            self._refuse_unused_capture()
             # a kernel that gave up on a stalled peer leaves undefined bucket contents: never train on them
             self.comm.check()
             self._reset_reducer_state()
@@ -316,6 +317,7 @@ class DistributedDataParallel(nn.Module):
         if not self.require_backward_grad_sync:
             return
         if not self._callback_queued:
+            self._refuse_unused_capture()  # a backward captured on its own, after an eager forward
             self._callback_queued = True
             torch.autograd.Variable._execution_engine.queue_callback(self._finalize_backward)
             if self.find_unused_parameters:
@@ -326,6 +328,15 @@ class DistributedDataParallel(nn.Module):
                 "a parameter that the forward's output does not reach produced a gradient: it was already marked ready as "
                 "unused.  Compute the loss only from the DistributedDataParallel output")
         self._mark_ready(p)
+
+    def _refuse_unused_capture(self) -> None:
+        """find_unused_parameters needs the host: the backward copies the locally used map from pageable memory and waits
+        for its reduction before it knows which .grad to keep.  Neither can be captured in a CUDA graph, so a synced
+        forward or backward under capture raises here, before any bucket is launched."""
+        if self.find_unused_parameters and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError(
+                "find_unused_parameters=True cannot run under CUDA graph capture: the parameters no rank used are known "
+                "only after a host wait for the reduced used map; capture with find_unused_parameters=False")
 
     def _mark_ready(self, p: nn.Parameter) -> None:
         b = self._bucket_of[id(p)]
@@ -414,6 +425,8 @@ class DistributedDataParallel(nn.Module):
         scale, order and stream of the allreduce.  Its gradients are read in place, or copied into one scratch tensor
         first when they cannot be (more segments than a table holds, another layout, zero_copy=False)."""
         zero = self._step_in_backward
+        if zero is not None:
+            zero._refuse_capture()
         if self._next_bucket == 0 and zero is not None and zero._stepped_in_backward:
             # the parameters of this rank's blocks already hold the update of the previous backward: a second update
             # before step() all-gathers it would step from a half-updated model.  Raised before any bucket is launched.

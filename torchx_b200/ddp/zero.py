@@ -243,6 +243,17 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
                     st["exp_avg_sq"] = self._flat_state[bi]["exp_avg_sq"][lo:hi]
                 self.optim.state[v] = st
 
+    @staticmethod
+    def _refuse_capture() -> None:
+        """Overlap mode under CUDA graph capture.  The fused step takes every run's step count (Adam's bias correction,
+        SGD's first-step rule) and every group's lr as launch parameters, and step() advances the counts on the host: a
+        replay would repeat the captured step's values forever.  Raised before the first bucket launch of a captured
+        backward, and by a captured step()."""
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError(
+                "overlap_with_ddp=True cannot be captured in a CUDA graph: the step counts and lr are launch parameters of "
+                "the fused step, so every replay would repeat the captured step; capture without overlap_with_ddp")
+
     def _launch_table(self, b) -> "N.B2Optim":
         """The b2_optim_t of one bucket launch: this rank's parameter (or master) and state blocks, its runs (adjacent parameters of
         one group and step count coalesced) and every group's hyper-parameters as param_groups hold them now."""
@@ -325,6 +336,7 @@ class ZeroRedundancyOptimizer(torch.optim.Optimizer):
             raise RuntimeError(
                 "overlap_with_ddp=True does not support GradScaler: dynamic loss scaling needs the rank-global found-inf "
                 "before any update, and with overlap the update has already happened during backward")
+        self._refuse_capture()
         if not self._stepped_in_backward:
             return None
         self._stepped_in_backward = False
