@@ -195,6 +195,10 @@ class DistributedDataParallel(nn.Module):
             for p in b.params:
                 self._bucket_of[id(p)] = b
         self._comm_stream = torch.cuda.Stream(device=self.device)
+        prev = self.comm.ordered_stream
+        if prev is not None:  # collectives already queued on the previous owner's stream (a b200 process group's) run first
+            self._comm_stream.wait_stream(prev)
+            torch.cuda.current_stream(self.device).wait_stream(prev)
         # bucket allreduces run on this stream mid-backward: other collectives of the communicator (SyncBatchNorm) join it
         self.comm.ordered_stream = self._comm_stream
         self._ready_event = torch.cuda.Event()
@@ -234,6 +238,8 @@ class DistributedDataParallel(nn.Module):
         channels_last and contiguous replicas agree)."""
         if self.world_size == 1 or not tensors:
             return
+        from torchx_b200.nn.batchnorm import _ordered
+
         by_dtype: Dict[torch.dtype, List[torch.Tensor]] = {}
         for t in tensors:
             by_dtype.setdefault(t.dtype, []).append(t)
@@ -249,7 +255,9 @@ class DistributedDataParallel(nn.Module):
                 size += nbytes
             for chunk in chunks:
                 flat = torch.cat([t.detach().reshape(-1) for t in chunk])
-                self.comm.broadcast_(flat, root=0)
+                # on the ordered stream, after (and before) whatever the communicator already has queued there, e.g. a
+                # b200 process group's async collectives the caller has not waited for yet (DESIGN.md 2.7)
+                _ordered(self.comm, lambda s, flat=flat: self.comm.broadcast_(flat, root=0, stream=s))
                 if self.comm.rank != 0:
                     outs = torch.split(flat, [t.numel() for t in chunk])
                     torch._foreach_copy_([t.detach() for t in chunk], [o.view_as(t) for o, t in zip(outs, chunk)])

@@ -35,11 +35,13 @@ class B200HookState:
 def _run(state: B200HookState, bucket, wire: str) -> torch.futures.Future[torch.Tensor]:
     buf = bucket.buffer()
     cur = torch.cuda.current_stream(state.device)
+    # under a b200 process group every collective of the communicator runs on its ordered stream (DESIGN.md 2.7)
+    stream = state.comm.ordered_stream if state.comm.ordered_stream is not None else state.stream
     state.event.record(cur)  # the Reducer filled the bucket on the backward stream
-    state.stream.wait_event(state.event)
-    state.comm.allreduce_(buf, scale=1.0 / state.comm.world, wire=wire, algo=state.algo, stream=state.stream)
+    stream.wait_event(state.event)
+    state.comm.allreduce_(buf, scale=1.0 / state.comm.world, wire=wire, algo=state.algo, stream=stream)
     fut: torch.futures.Future[torch.Tensor] = torch.futures.Future(devices=[state.device])
-    with torch.cuda.stream(state.stream):
+    with torch.cuda.stream(stream):
         fut.set_result(buf)  # the CUDA future captures an event on state.stream; fut.wait() orders consumers after it
     return fut
 

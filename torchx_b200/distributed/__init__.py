@@ -61,12 +61,12 @@ def local_cuda_device() -> torch.device:
 
 def local_device() -> torch.device:
     """The device this process should place its model on: ``cuda:<pinned ordinal>`` when the native communicator or an
-    nccl process group is active, ``cpu`` under any other process group; with nothing initialised, ``cuda`` if the host
-    has GPUs else ``cpu`` (reference torchx/distributed/__init__.py:70-88)."""
+    nccl or b200 process group is active, ``cpu`` under any other process group; with nothing initialised, ``cuda`` if
+    the host has GPUs else ``cpu`` (reference torchx/distributed/__init__.py:70-88)."""
     if _COMM is not None:
         return torch.device("cuda", _COMM.device)
     if dist.is_available() and dist.is_initialized():
-        return local_cuda_device() if dist.get_backend() == "nccl" else torch.device("cpu")
+        return local_cuda_device() if dist.get_backend() in ("nccl", "b200") else torch.device("cpu")
     return torch.device("cuda") if has_cuda_devices() else torch.device("cpu")
 
 
@@ -225,9 +225,9 @@ def broadcast(tensor: torch.Tensor, src: int, group: Any = None, async_op: bool 
     return None
 
 
-def _split_rows(t: torch.Tensor, sizes: Optional[List[int]], what: str) -> List[torch.Tensor]:
+def _split_rows(t: torch.Tensor, sizes: Optional[List[int]], what: str, world: Optional[int] = None) -> List[torch.Tensor]:
     """``t`` cut along its first dimension into world views: ``sizes`` rows each, or evenly when ``sizes`` is None / empty."""
-    world = _COMM.world
+    world = _COMM.world if world is None else world
     if not sizes:
         if t.size(0) % world:
             raise ValueError(f"all_to_all_single: {what} has {t.size(0)} rows, not a multiple of the world size {world}; "
@@ -423,9 +423,10 @@ def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = N
     return None
 
 
-def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor) -> None:
-    if len(tensors) != _COMM.world:
-        raise ValueError(f"{what} has {len(tensors)} tensors, world size is {_COMM.world}")
+def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor, world: Optional[int] = None) -> None:
+    world = _COMM.world if world is None else world
+    if len(tensors) != world:
+        raise ValueError(f"{what} has {len(tensors)} tensors, world size is {world}")
     for t in tensors:
         if t.dtype != like.dtype or t.numel() != like.numel():
             raise ValueError(f"{what}: every tensor must be {like.dtype} with {like.numel()} elements")
@@ -672,3 +673,9 @@ def on_local_rank0_first() -> Iterator[None]:
     finally:
         if first:
             barrier()
+
+
+# ``dist.init_process_group("b200")``: the native communicator as a torch.distributed backend (_backend.py)
+from torchx_b200.distributed._backend import B200ProcessGroup, register_backend  # noqa: E402
+
+register_backend()
