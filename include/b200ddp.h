@@ -27,6 +27,8 @@
  *   b2_allreduce_gather <- the Reducer's bucket copy-in fused into the hook (reducer.cpp mark_variable_ready_dense)
  *   b2_broadcast       <- DDP init / per-forward buffer sync torch/nn/parallel/distributed.py:881-890, 2176-2243
  *   b2_barrier         <- dist.barrier()                     torchx/distributed/__init__.py:268,274,297,303
+ *   b2_comm_create_group <- dist.new_group(ranks) / dist.new_subgroups*  (a communicator over a subset of an existing
+ *                         one's ranks: a control block named after the parent's, no second launcher rendezvous)
  *   b2_comm_destroy    <- dist.destroy_process_group()
  *
  * Conventions: plain pointers and sizes only (no torch types); every function returns
@@ -52,7 +54,7 @@ extern "C" {
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
                             b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats,
-                            b2_bn_backward_reduce, b2_reduce and b2_reduce_scatter_step_bf16, which only add symbols: a binding that needs them
+                            b2_bn_backward_reduce, b2_reduce, b2_reduce_scatter_step_bf16 and b2_comm_create_group, which only add symbols: a binding that needs them
                             fails to resolve them against an older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -128,6 +130,31 @@ int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char*
  * distinct devices it uses cudaDeviceEnablePeerAccess instead of CUDA IPC.
  */
 int b2_comm_create_local(b2_comm_t** out, int world, const int* devices, size_t stage_bytes);
+
+/*
+ * Create a communicator over a subset of `parent`'s ranks (MPI_Comm_create, torch's new_group).  Collective over every rank
+ * of `parent`: all of them call it, in the same order relative to their other b2_comm_create_group calls on `parent`.
+ * `ranks` holds `n_ranks` parent ranks in increasing order without duplicates; a member's rank in the group is its index in
+ * `ranks`.  A non-member gets *out = NULL and B2_OK and touches no shared memory.
+ *   - Naming: the group's control block is "<parent's control block name>.g<k>", k = the number of earlier calls on
+ *     `parent` (every call advances it on every rank, members or not), so no two groups ever share a block.
+ *   - Validation: the first member to arrive records the parent's world and `ranks` in the block and every other member
+ *     compares, so member lists that differ between ranks are B2_EINVAL on the members that meet, not a timeout.  B2_EINVAL
+ *     before any allocation for: a null `out` or `parent`, a parent from b2_comm_create_local (create an in-process world
+ *     over the member devices instead), n_ranks outside 1..parent's world, a null `ranks`, and unsorted, duplicate or out
+ *     of range ranks; B2_ESTATE for a poisoned parent.
+ *   - Settings: the device and the in-kernel timeout are the parent's.  The AUTO policy, grids and tuning knobs are the
+ *     defaults b2_comm_create gives a world of n_ranks (with its environment overrides): b2_comm_set_param /
+ *     b2_comm_set_max_ctas calls on the parent do not carry over.  stage_bytes == 0 means B2_GROUP_STAGE_MB MiB.  The
+ *     rendezvous is bounded by the parent's creation timeout.  A one-member group is a world of one with no shared memory.
+ *   - Lifetime: the group is independent of `parent` once created; either may be destroyed first.  No shm object is left
+ *     behind, on success or on failure.
+ * While a process holds two or more communicators of b2_comm_create / b2_comm_create_group with more than one rank, their
+ * launches run in one process-wide order (host issue order); collectives of communicators that share ranks must then be
+ * issued in the same relative order on those ranks, as torch requires of overlapping process groups (DESIGN.md 2.8).
+ */
+#define B2_GROUP_STAGE_MB 64
+int b2_comm_create_group(b2_comm_t** out, const b2_comm_t* parent, int n_ranks, const int* ranks, size_t stage_bytes);
 
 int b2_comm_destroy(b2_comm_t* comm);
 

@@ -129,6 +129,13 @@ struct ShmBlock {
   std::atomic<int> mc_mapped;  // ... past mapping the multicast object
   std::atomic<int> mc_fail;    // any rank failed a multicast step: everybody drops the NVLS path
   ShmSlot slot[B2_MAX_WORLD];
+  // group communicators (b2_comm_create_group): the first member to arrive records its parent's world and the member
+  // list; every later member compares and, on a difference, sets `group_bad`, which ends every member's rendezvous
+  std::atomic<int> group_state;  // 0: empty, 1: being recorded, 2: recorded
+  std::atomic<int> group_bad;
+  int group_parent_world;
+  int group_n;
+  int group_ranks[B2_MAX_WORLD];
 };
 
 // the multicast mapping of an in-process world is shared by its ranks
@@ -176,6 +183,12 @@ struct b2_comm {
   int last_algo = 0;                  // B2_ALGO_* of the most recent allreduce launch (what AUTO picked)
   ShmBlock* shm = nullptr;
   std::string shm_path;
+  // host-only: where b2_comm_create_group derives its groups' control blocks from
+  std::string shm_base;      // the name b2_comm_create was given (a group: its parent's control block name)
+  uint64_t epoch = 0;
+  unsigned groups_made = 0;  // b2_comm_create_group calls on this communicator, members or not
+  int rdv_timeout_ms = 0;    // the rendezvous bound it was created with
+  bool ordered = false;      // one rank per process over shm (not local_world, W > 1): takes part in LaunchOrder
 };
 
 namespace {
@@ -568,6 +581,8 @@ bool wait_count(std::atomic<int>& ctr, int target, std::atomic<int>* abort_flag,
 int wait_slots(const b2_comm* c, std::atomic<uint32_t> ShmSlot::*flag, double deadline) {
   for (int r = 0; r < c->d.world; ++r) {
     while ((c->shm->slot[r].*flag).load(std::memory_order_acquire) != 1) {
+      if (c->shm->group_bad.load(std::memory_order_acquire))
+        return fail(B2_EINVAL, "b2_comm_create_group: the members passed different rank lists (%s)", c->shm_path.c_str());
       if (now_s() > deadline) return fail(B2_ETIMEOUT, "rendezvous timed out waiting for rank %d on %s", r, c->shm_path.c_str());
       usleep(200);
     }
@@ -592,6 +607,40 @@ int check_not_poisoned(const b2_comm* c) {
   if (s != 0) return fail(B2_ESTATE, "communicator poisoned by an earlier peer-wait timeout");
   return B2_OK;
 }
+
+// One process-wide order for the launches of every communicator that has one rank per process (DESIGN.md 2.8).  While
+// the process holds two or more of them (a world and its groups, say), each multi-rank launch waits on the stream it is
+// issued on for the previous such launch of the process, whichever communicator and stream that was.  A rank's fabric
+// kernels then run one after another in host issue order, so they never compete for SMs while waiting on peers, and the
+// only possible cycle is a caller's: collectives of overlapping communicators issued in different relative orders on
+// the ranks they share.  Inside a CUDA graph capture the order is left to the graph's own dependencies.
+std::atomic<int> g_ordered_comms{0};
+std::mutex g_order_mu;
+cudaEvent_t g_order_ev[64] = {};  // per device: cudaEventRecord needs an event of the stream's device
+cudaEvent_t g_order_last = nullptr;
+
+struct LaunchOrder {
+  cudaStream_t s = nullptr;
+  int dev = -1;
+  LaunchOrder(const b2_comm* c, void* stream) {
+    if (!c->ordered || g_ordered_comms.load(std::memory_order_acquire) < 2 || c->device < 0 || c->device >= 64) return;
+    s = static_cast<cudaStream_t>(stream);
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(s, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+      cudaGetLastError();
+      return;
+    }
+    g_order_mu.lock();
+    dev = c->device;
+    if (g_order_last) cudaStreamWaitEvent(s, g_order_last, 0);
+  }
+  ~LaunchOrder() {
+    if (dev < 0) return;
+    if (!g_order_ev[dev]) cudaEventCreateWithFlags(&g_order_ev[dev], cudaEventDisableTiming);
+    if (g_order_ev[dev] && cudaEventRecord(g_order_ev[dev], s) == cudaSuccess) g_order_last = g_order_ev[dev];
+    g_order_mu.unlock();
+  }
+};
 
 // Multi-process multicast bring-up (after every rank has mapped every peer arena).  Any failure on any rank sets
 // sb->mc_fail and every rank drops the NVLS path together; the P2P mappings are unaffected.
@@ -792,29 +841,56 @@ int b2_comm_create_local(b2_comm_t** out, int world, const int* devices, size_t 
   return rc;
 }
 
-int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char* shm_name,
-                   uint64_t epoch, size_t stage_bytes, int timeout_ms) {
-  if (!out || world < 1 || world > B2_MAX_WORLD || rank < 0 || rank >= world || device < 0)
-    return fail(B2_EINVAL, "b2_comm_create: bad arguments (rank=%d world=%d device=%d)", rank, world,
-                device);
-  if (world > 1 && (!shm_name || !*shm_name))
-    return fail(B2_EINVAL, "b2_comm_create: shm_name is required when world > 1");
+}  // extern "C"
+
+namespace {
+
+// What a group member checks against the control block (b2_comm_create_group).
+struct GroupRecord {
+  int parent_world;
+  int n;
+  const int* ranks;
+};
+
+// The first member records `g`; every other member waits for the record and compares.  A difference sets group_bad, which
+// every member's rendezvous wait sees.
+int check_group_record(b2_comm* c, const GroupRecord& g, double deadline) {
+  ShmBlock* sb = c->shm;
+  int expect = 0;
+  if (sb->group_state.compare_exchange_strong(expect, 1, std::memory_order_acq_rel)) {
+    sb->group_parent_world = g.parent_world;
+    sb->group_n = g.n;
+    for (int i = 0; i < g.n; ++i) sb->group_ranks[i] = g.ranks[i];
+    sb->group_state.store(2, std::memory_order_release);
+    return B2_OK;
+  }
+  while (sb->group_state.load(std::memory_order_acquire) != 2) {
+    if (now_s() > deadline) return fail(B2_ETIMEOUT, "rendezvous timed out waiting for the group record on %s", c->shm_path.c_str());
+    usleep(200);
+  }
+  bool same = sb->group_parent_world == g.parent_world && sb->group_n == g.n;
+  for (int i = 0; same && i < g.n; ++i) same = sb->group_ranks[i] == g.ranks[i];
+  if (same) return B2_OK;
+  sb->group_bad.store(1, std::memory_order_release);
+  return fail(B2_EINVAL, "b2_comm_create_group: the members passed different rank lists (%s)", c->shm_path.c_str());
+}
+
+// b2_comm_create once the control block's name `path` is known (unused at world == 1); `group` is non-null for a group
+// member, whose failures unlink the name on every member so that no shm object outlives a failed rendezvous.
+int create_comm(b2_comm_t** out, int rank, int world, int device, const char* path, uint64_t epoch, size_t stage_bytes, int timeout_ms,
+                const GroupRecord* group) {
   const double deadline = now_s() + (timeout_ms > 0 ? timeout_ms : 120000) * 1e-3;
   int prev = -1;
   cudaGetDevice(&prev);
   b2_comm* c = new (std::nothrow) b2_comm();
   if (!c) return fail(B2_ESYS, "out of host memory");
+  c->rdv_timeout_ms = timeout_ms;
+  c->epoch = epoch;
   int rc = init_rank(c, rank, world, device, stage_bytes);
   int sock = -1;
   std::string sock_base;
   if (rc == B2_OK && world == 1) rc = alloc_arena(c, false, false, &device, 1);
   if (rc == B2_OK && world > 1) {
-    // <name>.e<epoch>.c<n>: n counts this process's communicators on (name, epoch).  Every rank creates its
-    // communicators in the same order, so n agrees across ranks, and a second communicator (init_pg + DDP, two DDP
-    // modules) can never open the control block of the first one while rank 0 has not unlinked it yet.
-    char path[256];
-    snprintf(path, sizeof(path), "%s%s.e%llu.c%u", shm_name[0] == '/' ? "" : "/", shm_name,
-             static_cast<unsigned long long>(epoch), next_creation_index(shm_name, epoch));
     c->shm_path = path;
     sock_base = std::string("b2fd") + path;
     int fd = shm_open(path, O_CREAT | O_RDWR, 0600);
@@ -829,6 +905,7 @@ int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char*
         c->shm = static_cast<ShmBlock*>(m);
     }
     if (fd >= 0) close(fd);
+    if (rc == B2_OK && group) rc = check_group_record(c, *group, deadline);
   }
   if (rc == B2_OK && world > 1) {
     ShmBlock* sb = c->shm;
@@ -977,20 +1054,90 @@ int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char*
     for (int r = 0; r < world; ++r)
       if (c->peer_is_ipc[r]) cudaIpcCloseMemHandle(c->arena_of[r]);
     if (c->shm) munmap(c->shm, sizeof(ShmBlock));
-    if (rank == 0 && !c->shm_path.empty()) shm_unlink(c->shm_path.c_str());
+    if ((rank == 0 || group) && !c->shm_path.empty()) shm_unlink(c->shm_path.c_str());
     free_rank_resources(c);
     delete c;
     g_err = keep;
   } else {
     rotate_peers(c);
+    if (world > 1) {
+      c->ordered = true;
+      g_ordered_comms.fetch_add(1, std::memory_order_acq_rel);
+    }
     *out = c;
   }
   if (prev >= 0) cudaSetDevice(prev);
   return rc;
 }
 
+}  // namespace
+
+extern "C" {
+
+int b2_comm_create(b2_comm_t** out, int rank, int world, int device, const char* shm_name,
+                   uint64_t epoch, size_t stage_bytes, int timeout_ms) {
+  if (!out || world < 1 || world > B2_MAX_WORLD || rank < 0 || rank >= world || device < 0)
+    return fail(B2_EINVAL, "b2_comm_create: bad arguments (rank=%d world=%d device=%d)", rank, world,
+                device);
+  if (world > 1 && (!shm_name || !*shm_name))
+    return fail(B2_EINVAL, "b2_comm_create: shm_name is required when world > 1");
+  // <name>.e<epoch>.c<n>: n counts this process's communicators on (name, epoch).  Every rank creates its
+  // communicators in the same order, so n agrees across ranks, and a second communicator (init_pg + DDP, two DDP
+  // modules) can never open the control block of the first one while rank 0 has not unlinked it yet.
+  char path[256] = {};
+  if (world > 1)
+    snprintf(path, sizeof(path), "%s%s.e%llu.c%u", shm_name[0] == '/' ? "" : "/", shm_name,
+             static_cast<unsigned long long>(epoch), next_creation_index(shm_name, epoch));
+  const int rc = create_comm(out, rank, world, device, path, epoch, stage_bytes, timeout_ms, nullptr);
+  if (rc == B2_OK) (*out)->shm_base = path;
+  return rc;
+}
+
+int b2_comm_create_group(b2_comm_t** out, const b2_comm_t* parent, int n_ranks, const int* ranks, size_t stage_bytes) {
+  if (!out) return fail(B2_EINVAL, "b2_comm_create_group: null out");
+  *out = nullptr;
+  if (!parent) return fail(B2_EINVAL, "b2_comm_create_group: null parent");
+  if (parent->local_world)
+    return fail(B2_EINVAL, "b2_comm_create_group: the parent is an in-process world; call b2_comm_create_local over the member devices");
+  if (const int rc = check_not_poisoned(parent)) return rc;
+  const int PW = parent->d.world;
+  if (n_ranks < 1 || n_ranks > PW)
+    return fail(B2_EINVAL, "b2_comm_create_group: n_ranks=%d outside 1..%d (the parent's world)", n_ranks, PW);
+  if (!ranks) return fail(B2_EINVAL, "b2_comm_create_group: null ranks");
+  int me = -1;
+  for (int i = 0; i < n_ranks; ++i) {
+    if (ranks[i] < 0 || ranks[i] >= PW)
+      return fail(B2_EINVAL, "b2_comm_create_group: rank %d is not a rank of the parent's world of %d", ranks[i], PW);
+    if (i > 0 && ranks[i] <= ranks[i - 1])
+      return fail(B2_EINVAL, "b2_comm_create_group: ranks must be increasing without duplicates (%d after %d)", ranks[i], ranks[i - 1]);
+    if (ranks[i] == parent->d.rank) me = i;
+  }
+  if (stage_bytes == 0) stage_bytes = static_cast<size_t>(B2_GROUP_STAGE_MB) << 20;
+  // every rank of the parent advances the counter, members or not, so it agrees across the parent's ranks
+  b2_comm* p = const_cast<b2_comm*>(parent);
+  const unsigned k = p->groups_made++;
+  if (me < 0) return B2_OK;
+  // <parent's control block name>.g<k>: unique per parent and call, whatever the member lists
+  char path[256] = {};
+  if (n_ranks > 1) {
+    const int len = snprintf(path, sizeof(path), "%s.g%u", parent->shm_base.c_str(), k);
+    if (len < 0 || static_cast<size_t>(len) >= sizeof(path) || parent->shm_base.empty())
+      return fail(B2_EINVAL, "b2_comm_create_group: no control block name for a group of %s", parent->shm_base.c_str());
+  }
+  const GroupRecord rec{PW, n_ranks, ranks};
+  const int rc = create_comm(out, me, n_ranks, parent->device, path, parent->epoch, stage_bytes, parent->rdv_timeout_ms, &rec);
+  if (rc != B2_OK) {
+    *out = nullptr;
+    return rc;
+  }
+  (*out)->shm_base = path;
+  (*out)->d.timeout_ns = parent->d.timeout_ns;
+  return B2_OK;
+}
+
 int b2_comm_destroy(b2_comm_t* c) {
   if (!c) return B2_OK;
+  if (c->ordered) g_ordered_comms.fetch_sub(1, std::memory_order_acq_rel);
   int prev = -1;
   cudaGetDevice(&prev);
   cudaSetDevice(c->device);
@@ -1124,6 +1271,7 @@ static int allreduce_impl(b2_comm_t* c, Src& src, void* buf, size_t n_elems, int
   if (algo == B2_ALGO_NVLS && c->d.mc == nullptr)
     return fail(B2_ENOTSUP, "B2_ALGO_NVLS: this communicator has no multicast mapping (b2_comm_caps)");
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t wvb = wire_vec_bytes(mode);
   const size_t cap_vecs = c->d.slice_cap / wvb;  // vecs one region can hold
@@ -1209,6 +1357,7 @@ int b2_reduce_scatter_gather(b2_comm_t* c, void* out, size_t block, const b2_seg
     return rc;
   }
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t eb = elem_bytes(mode);
   const size_t cap = c->d.slice_cap / wire_vec_bytes(mode) * 8;  // elements of a block one recv region holds (whole vecs)
@@ -1325,6 +1474,7 @@ int b2_reduce_scatter_step(b2_comm_t* c, size_t block, const b2_segment_t* segme
   if (const int rc = segment_table("b2_reduce_scatter_step", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaError_t e = cudaErrorInvalidValue;
   with_mode(mode, [&](auto m) {
     constexpr int MODE = decltype(m)::value;
@@ -1349,6 +1499,7 @@ int b2_reduce_scatter_step_bf16(b2_comm_t* c, size_t block, const b2_segment_t* 
   if (const int rc = segment_table("b2_reduce_scatter_step_bf16", segments, n_segments, static_cast<size_t>(W) * block, src)) return rc;
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   const cudaError_t e = launch_step<B2_BF16>(c, src, o, block, scale, stream);
   if (e != cudaSuccess) return fail(B2_ECUDA, "reduce-scatter step kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
@@ -1361,6 +1512,7 @@ int b2_broadcast(b2_comm_t* c, void* buf, size_t bytes, int root, void* stream) 
   if (!buf) return fail(B2_EINVAL, "b2_broadcast: null buffer");
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t cap = c->stage_bytes & ~static_cast<size_t>(15);
   const cudaError_t e = for_chunks(c, bytes, cap, [&](size_t off, size_t n) {
@@ -1472,6 +1624,7 @@ int b2_allreduce_op(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, 
     return allreduce_impl(c, src, buf, n_elems, mode, op == B2_OP_AVG ? 1.0f / static_cast<float>(W) : 1.0f, B2_ALGO_AUTO, stream);
   }
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t eb = dtype_bytes(dtype);
   const size_t cap = c->d.slice_cap / eb;  // elements one recv region holds (slice_cap is a multiple of 256 bytes)
@@ -1492,6 +1645,7 @@ int b2_allgather(b2_comm_t* c, void* out, const void* in, size_t bytes, void* st
     return fail(B2_EINVAL, "b2_allgather: `in` overlaps `out` other than as this rank's block");
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (W == 1) {
     if (!in_place) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
@@ -1519,6 +1673,7 @@ int b2_reduce_scatter(b2_comm_t* c, void* out, const void* in, size_t n_elems, i
     return fail(B2_EINVAL, "b2_reduce_scatter: `out` overlaps `in` other than as this rank's block");
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (W == 1) {
     if (!in_place) B2_CUDA(cudaMemcpyAsync(out, in, bytes, cudaMemcpyDeviceToDevice, s));
@@ -1562,6 +1717,7 @@ int b2_reduce(b2_comm_t* c, void* buf, size_t n_elems, int dtype, int op, int ro
   if (const int rc = check_not_poisoned(c)) return rc;
   if (W == 1) return B2_OK;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool sum = !dtype_is_int(dtype) && (op == B2_OP_SUM || op == B2_OP_AVG);
   const int mode = sum_mode_for(dtype);
@@ -1615,6 +1771,7 @@ int b2_alltoall(b2_comm_t* c, void* const* out, const size_t* recv_bytes, const 
   }
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (W == 1) {
     if (send_bytes[0] != recv_bytes[0])
@@ -1710,6 +1867,7 @@ int b2_p2p(b2_comm_t* c, const b2_p2p_op_t* ops, int n_ops, void* stream) {
   a.status = c->d.status;
   a.timeout_ns = c->d.timeout_ns;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   k_p2p<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(a);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "point-to-point kernel launch: %s", cudaGetErrorString(e));
@@ -1729,6 +1887,7 @@ int b2_batchnorm_stats(b2_comm_t* c, float* mean, float* invstd, float count, si
                 c->d.slice_cap);
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   // ATen's kernel takes eps and momentum as float parameters: the same double -> float conversion as at its launch
   k_bn_stats<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(c->d, mean, invstd, count, channels, running_mean, running_var,
                                                                     static_cast<float>(momentum), static_cast<float>(eps), counts_out);
@@ -1901,6 +2060,7 @@ int b2_barrier(b2_comm_t* c, void* stream) {
   if (c->d.world == 1) return B2_OK;
   if (const int rc = check_not_poisoned(c)) return rc;
   DeviceGuard g(c->device);
+  LaunchOrder order(c, stream);
   k_barrier<<<1, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(c->d);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "barrier kernel launch: %s", cudaGetErrorString(e));

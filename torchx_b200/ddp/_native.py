@@ -19,6 +19,7 @@ INCLUDE_DIR = os.path.join(os.path.dirname(_PKG), "include")
 
 B2_ABI_VERSION = 3
 B2_MAX_WORLD = 8
+B2_GROUP_STAGE_MB = 64
 
 B2_OK = 0
 B2_EINVAL = -1
@@ -121,6 +122,7 @@ SIGNATURES = {
     "b2_last_error": (ctypes.c_char_p, []),
     "b2_comm_create": (_i, [_P(_vp), _i, _i, _i, ctypes.c_char_p, _u64, _sz, _i]),
     "b2_comm_create_local": (_i, [_P(_vp), _i, _P(_i), _sz]),
+    "b2_comm_create_group": (_i, [_P(_vp), _vp, _i, _P(_i), _sz]),
     "b2_comm_destroy": (_i, [_vp]),
     "b2_comm_rank": (_i, [_vp]),
     "b2_comm_world": (_i, [_vp]),

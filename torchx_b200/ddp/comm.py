@@ -135,6 +135,33 @@ class Communicator:
         N.check(N.lib().b2_comm_create_local(outs, w, devs, stage_mb << 20))
         return [cls(outs[i]) for i in range(w)]
 
+    def create_group(self, ranks: Sequence[int], stage_mb: int = 0) -> Optional["Communicator"]:
+        """A communicator over the ranks ``ranks`` of this one (include/b200ddp.h: b2_comm_create_group), or None on a rank
+        outside them.  Every rank of this communicator calls it, in the same order as its other ``create_group`` calls;
+        ``ranks`` is increasing, without duplicates, and the same on every rank.  The result's ``rank`` is this rank's index in
+        ``ranks`` and its ``ranks`` the list itself, in this communicator's numbering (its own ``ranks`` when it is a group).
+        ``stage_mb`` 0 is ``B2_GROUP_STAGE_MB``.  It inherits the device and the in-kernel timeout, not ``set_param`` values."""
+        rs = [as_rank(r) for r in ranks]
+        if any(r is None for r in rs):
+            raise ValueError(f"create_group: ranks {list(ranks)!r} must be integers")
+        out = ctypes.c_void_p()
+        arr = (ctypes.c_int * max(len(rs), 1))(*rs)
+        N.check(N.lib().b2_comm_create_group(ctypes.byref(out), self._h, len(rs), arr, stage_mb << 20))
+        if not out.value:
+            return None
+        g = type(self)(out.value)
+        g.ranks = [self.ranks[r] for r in rs]
+        return g
+
+    @property
+    def ranks(self) -> List[int]:
+        """The global ranks of this communicator, by its rank: ``range(world)`` unless it was made by ``create_group``."""
+        return self.__dict__.get("_ranks") or list(range(self.world))
+
+    @ranks.setter
+    def ranks(self, value: List[int]) -> None:
+        self._ranks = list(value)
+
     def close(self) -> None:
         if self._h and self._owner:
             N.lib().b2_comm_destroy(self._h)

@@ -12,7 +12,8 @@ environment contract and barrier-ordered critical sections.  Two backends behind
     ``isend``, ``irecv``, ``P2POp`` / ``batch_isend_irecv``, ``gather`` / ``scatter``, ``reduce`` to a root and the object
     collectives ``all_gather_object``, ``broadcast_object_list``, ``gather_object``, ``scatter_object_list``,
     ``send_object_list`` / ``recv_object_list`` then run on that fabric.  The object collectives unpickle what peers send,
-    so they trust every peer, as torch's do.
+    so they trust every peer, as torch's do.  ``new_group``, ``new_subgroups`` and ``new_subgroups_by_enumeration`` make
+    ``B200Group``s, each with its own communicator over a subset of the ranks, which every helper takes as ``group=``.
 """
 from __future__ import annotations
 
@@ -117,13 +118,17 @@ def init_pg(backend: str = "auto", **kwargs: Any) -> torch.device:
     return local_cuda_device() if backend == "nccl" else torch.device("cpu")
 
 
-def barrier() -> None:
+def barrier(group: Any = None) -> None:
+    """A host-blocking barrier over the world, or over ``group`` (a ``B200Group``) under ``init_pg("b200")``."""
     if _COMM is not None and not dist.is_initialized():
-        _COMM.barrier()
-        torch.cuda.current_stream(_COMM.device).synchronize()
-        _COMM.check()  # a barrier kernel that gave up on a stalled peer must not let this rank into the critical section
+        comm = _comm_for(group)
+        if comm is None:
+            return _not_in_group("barrier")
+        comm.barrier()
+        torch.cuda.current_stream(comm.device).synchronize()
+        comm.check()  # a barrier kernel that gave up on a stalled peer must not let this rank into the critical section
     elif dist.is_initialized():
-        dist.barrier()
+        dist.barrier() if group is None else dist.barrier(group=group)
 
 
 def _on_fabric() -> bool:
@@ -131,11 +136,197 @@ def _on_fabric() -> bool:
     return _COMM is not None and not dist.is_initialized()
 
 
+class B200Group:
+    """A group of ranks of the native communicator (``new_group``): ``comm`` is its own communicator, whose rank is this
+    process's index in ``ranks`` (the members' global ranks, increasing).  Every helper of this module takes it as
+    ``group=``; ``src`` / ``dst`` / ``peer`` are then global ranks and ``group_src`` / ``group_dst`` / ``group_peer`` ranks of
+    the group, as in torch.distributed."""
+
+    def __init__(self, comm: Any, ranks: List[int]) -> None:
+        self.comm = comm
+        self.ranks = list(ranks)
+
+    def rank(self) -> int:
+        return self.comm.rank
+
+    def size(self) -> int:
+        return len(self.ranks)
+
+    def get_group_rank(self, global_rank: Any) -> int:
+        from torchx_b200.ddp.comm import as_rank
+
+        r = as_rank(global_rank)
+        if r is None or r not in self.ranks:
+            raise ValueError(f"Global rank {global_rank!r} is not part of group {self.ranks}")
+        return self.ranks.index(r)
+
+    def get_global_rank(self, group_rank: Any) -> int:
+        from torchx_b200.ddp.comm import as_rank
+
+        r = as_rank(group_rank)
+        if r is None or not 0 <= r < len(self.ranks):
+            raise ValueError(f"Group rank {group_rank!r} is not part of group {self.ranks}")
+        return self.ranks[r]
+
+    def __repr__(self) -> str:
+        return f"B200Group(ranks={self.ranks})"
+
+
+NON_GROUP_MEMBER = dist.GroupMember.NON_GROUP_MEMBER  # what new_group returns on a rank outside the group, as torch does
+
+
+def _is_non_member(group: Any) -> bool:
+    return type(group) is int and group == NON_GROUP_MEMBER
+
+
+def new_group(ranks: Optional[List[int]] = None, stage_mb: Optional[int] = None) -> Any:
+    """``torch.distributed.new_group`` under ``init_pg("b200")``: a ``B200Group`` over the global ``ranks`` (any order; None
+    is every rank) on a member, ``NON_GROUP_MEMBER`` elsewhere.  Every rank calls it, with the same ranks, in the same order
+    as its other ``new_group`` calls.  The group's communicator has its own arena of 2 stages of ``stage_mb`` MiB (default
+    ``B2_GROUP_STAGE_MB``, DESIGN.md 2.8) and inherits the world's device and in-kernel timeout."""
+    if not _on_fabric():
+        raise RuntimeError('new_group: needs init_pg("b200") and no torch.distributed process group; with one, use '
+                           "torch.distributed.new_group")
+    from torchx_b200.ddp.comm import as_rank
+
+    W = _COMM.world
+    members = list(range(W)) if ranks is None else [as_rank(r) for r in ranks]
+    if any(r is None or not 0 <= r < W for r in members):
+        raise ValueError(f"new_group: ranks {list(ranks)!r} must be ranks of the world of {W}")
+    members = sorted(members)
+    if len(set(members)) != len(members):
+        raise ValueError(f"new_group: ranks {members} repeat a rank")
+    if not members:
+        raise ValueError("new_group: ranks is empty")
+    comm = _COMM.create_group(members, stage_mb or 0)
+    return NON_GROUP_MEMBER if comm is None else B200Group(comm, members)
+
+
+def new_subgroups_by_enumeration(ranks_per_subgroup_list: List[List[int]], timeout: Any = None, backend: Any = None,
+                                 pg_options: Any = None, group_desc: Any = None) -> Any:
+    """``torch.distributed.new_subgroups_by_enumeration``: one ``new_group`` per list, returns ``(the group of this rank or
+    None, every group)`` where a group this rank is not in is ``NON_GROUP_MEMBER``.  A rank in two lists is a ValueError.
+    ``timeout``, ``backend``, ``pg_options`` and ``group_desc`` are accepted and ignored."""
+    if not _on_fabric():
+        return dist.new_subgroups_by_enumeration(ranks_per_subgroup_list, timeout=timeout, backend=backend,
+                                                 pg_options=pg_options, group_desc=group_desc)
+    if ranks_per_subgroup_list is None or len(ranks_per_subgroup_list) == 0:
+        raise ValueError("The arg 'ranks_per_subgroup_list' cannot be empty")
+    seen = {}
+    for ranks in ranks_per_subgroup_list:  # checked before any group is made, so no rank is left in a half-made set
+        for r in ranks:
+            if r in seen:
+                raise ValueError(f"Rank {r} has appeared in both subgroup {seen[r]} and {ranks}")
+            seen[r] = ranks
+    subgroups, cur = [], None
+    for ranks in ranks_per_subgroup_list:
+        g = new_group(ranks)
+        subgroups.append(g)
+        if isinstance(g, B200Group):
+            cur = g
+    return cur, subgroups
+
+
+def new_subgroups(group_size: Optional[int] = None, group: Any = None, timeout: Any = None, backend: Any = None,
+                  pg_options: Any = None, group_desc: Any = None) -> Any:
+    """``torch.distributed.new_subgroups``: the ranks of ``group`` (None: the world) cut into consecutive groups of
+    ``group_size`` (default: the CUDA devices of this host), as ``new_subgroups_by_enumeration``."""
+    if not _on_fabric():
+        return dist.new_subgroups(group_size, group=group, timeout=timeout, backend=backend, pg_options=pg_options,
+                                  group_desc=group_desc)
+    if group_size is None:
+        if not torch.cuda.is_available():
+            raise ValueError("Default group size only takes effect when CUDA is available.If your subgroup using a backend "
+                             "that does not depend on CUDA,please pass in 'group_size' correctly.")
+        group_size = torch.cuda.device_count()
+    if group_size <= 0:
+        raise ValueError(f"The arg 'group_size' ({group_size}) must be positive")
+    if isinstance(group, B200Group):
+        ranks = group.ranks
+    elif group is None or group is dist.group.WORLD:
+        ranks = list(range(_COMM.world))
+    else:
+        raise NotImplementedError(_NO_SUBGROUPS)
+    if len(ranks) < group_size:
+        raise ValueError(f"The arg 'group_size' ({group_size}) must not exceed the world size ({len(ranks)})")
+    if len(ranks) % group_size != 0:
+        raise ValueError(f"The world size ({len(ranks)}) must be divisible by '{group_size=}'")
+    return new_subgroups_by_enumeration([ranks[i: i + group_size] for i in range(0, len(ranks), group_size)])
+
+
+_NO_SUBGROUPS = ("the b200 communicator has no subgroups but the B200Group of torchx_b200.distributed.new_group: pass "
+                 "group=None or a B200Group")
+
+
+def _comm_for(group: Any, async_op: bool = False) -> Any:
+    """The communicator a helper runs on: the world's for None / WORLD, the group's for a ``B200Group``, None for
+    ``NON_GROUP_MEMBER``.  Any other group, and ``async_op``, are refused."""
+    if group is None or group is dist.group.WORLD:
+        comm = _COMM
+    elif isinstance(group, B200Group):
+        comm = group.comm
+    elif _is_non_member(group):
+        comm = None
+    else:
+        raise NotImplementedError(_NO_SUBGROUPS)
+    if async_op:
+        raise NotImplementedError("the b200 communicator has no work handles: collectives are ordered on the current stream")
+    return comm
+
+
 def _check_native_call(group: Any, async_op: bool) -> None:
     if group is not None and group is not dist.group.WORLD:
         raise NotImplementedError("the b200 communicator has no subgroups: pass group=None")
     if async_op:
         raise NotImplementedError("the b200 communicator has no work handles: collectives are ordered on the current stream")
+
+
+def _not_in_group(op: str, ret: Any = None) -> Any:
+    """What torch.distributed does on a rank outside ``group``: warn and return (``_warn_not_in_group``)."""
+    warnings.warn(f"Running {op} on global rank {_COMM.rank} which does not belong to the given group.", stacklevel=3)
+    return ret
+
+
+def _group_rank(fn: str, name: str, group: Any, r: Any, group_r: Any, default: Optional[int] = 0) -> Any:
+    """The rank of ``group``'s communicator that a helper's ``name`` (a global rank) or ``group_name`` (a group rank)
+    names, as torch's ``_canonicalize_group_rank``: both given, a rank outside the group and, on ``NON_GROUP_MEMBER``, any
+    global rank are ValueErrors; on ``NON_GROUP_MEMBER`` a group rank is returned unchecked."""
+    if r is not None and group_r is not None:
+        raise ValueError(f"{fn}: Can't specify both group_{name} ({group_r!r}) and {name} ({r!r})")
+    if group_r is not None:
+        if _is_non_member(group):
+            return group_r
+        from torchx_b200.ddp.comm import as_rank
+
+        k = as_rank(group_r)
+        if k is None or not 0 <= k < group.comm.world:
+            raise ValueError(f"{fn}: group_{name} {group_r!r} is not a rank of a group of {group.comm.world}")
+        return k
+    if r is None:
+        if default is None:
+            raise ValueError(f"{fn}: {name} or group_{name} must be given")
+        r = default
+    if _is_non_member(group):
+        raise ValueError(f"{fn}: {name} {r!r} is a global rank, and this rank is not a member of the group to translate it")
+    return group.get_group_rank(r)
+
+
+def _world_rank(r: Any, group_r: Any) -> Any:
+    """``src`` / ``dst`` / ``peer`` on the world, where ``group_src`` ... is the same rank and may stand in for it."""
+    if group_r is None:
+        return r
+    if r is not None and r != group_r:
+        raise ValueError(f"group rank {group_r!r} differs from rank {r!r}; the world's group ranks are its ranks")
+    return group_r
+
+
+def _given(**kw: Any) -> dict:
+    """The keyword arguments that were given: a call delegated to torch.distributed passes the group_* ranks only then."""
+    return {k: v for k, v in kw.items() if v is not None}
+
+
+def _is_group(group: Any) -> bool:
+    return isinstance(group, B200Group) or _is_non_member(group)
 
 
 _REDUCE_OPS = ((dist.ReduceOp.SUM, "sum"), (dist.ReduceOp.AVG, "avg"), (dist.ReduceOp.MIN, "min"), (dist.ReduceOp.MAX, "max"))
@@ -155,8 +346,10 @@ def all_reduce(tensor: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = N
     With a process group it is ``torch.distributed.all_reduce``."""
     if not _on_fabric():
         return dist.all_reduce(tensor, op=op, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.allreduce_op_(tensor, reduce_op_name(op))
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("all_reduce")
+    comm.allreduce_op_(tensor, reduce_op_name(op))
     return None
 
 
@@ -166,8 +359,10 @@ def all_gather_into_tensor(output_tensor: torch.Tensor, input_tensor: torch.Tens
     along its first dimension (or, flat, as world consecutive blocks)."""
     if not _on_fabric():
         return dist.all_gather_into_tensor(output_tensor, input_tensor, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.allgather_(output_tensor, input_tensor)
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("all_gather_into_tensor")
+    comm.allgather_(output_tensor, input_tensor)
     return None
 
 
@@ -175,14 +370,16 @@ def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group: Any
     """``torch.distributed.all_gather``: ``tensor_list[r]`` <- rank r's ``tensor``."""
     if not _on_fabric():
         return dist.all_gather(tensor_list, tensor, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    if len(tensor_list) != _COMM.world:
-        raise ValueError(f"all_gather: tensor_list has {len(tensor_list)} tensors, world size is {_COMM.world}")
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("all_gather")
+    if len(tensor_list) != comm.world:
+        raise ValueError(f"all_gather: tensor_list has {len(tensor_list)} tensors, world size is {comm.world}")
     for t in tensor_list:
         if t.dtype != tensor.dtype or t.numel() != tensor.numel():
             raise ValueError(f"all_gather: every tensor of tensor_list must be {tensor.dtype} with {tensor.numel()} elements")
-    flat = torch.empty((_COMM.world,) + tuple(tensor.shape), dtype=tensor.dtype, device=tensor.device)
-    _COMM.allgather_(flat, tensor.contiguous())
+    flat = torch.empty((comm.world,) + tuple(tensor.shape), dtype=tensor.dtype, device=tensor.device)
+    comm.allgather_(flat, tensor.contiguous())
     for r, t in enumerate(tensor_list):
         t.copy_(flat[r].view_as(t))
     return None
@@ -195,8 +392,10 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, op: Any = d
     block r of what ``all_reduce`` with the same op leaves, bit for bit, at (W-1)/W of the input's bytes per rank."""
     if not _on_fabric():
         return dist.reduce_scatter_tensor(output, input, op=op, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.reduce_scatter_(output, input, reduce_op_name(op))
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("reduce_scatter_tensor")
+    comm.reduce_scatter_(output, input, reduce_op_name(op))
     return None
 
 
@@ -205,23 +404,32 @@ def reduce_scatter(output: torch.Tensor, input_list: List[torch.Tensor], op: Any
     """``torch.distributed.reduce_scatter``: rank r's ``output`` <- the reduction over ranks of their ``input_list[r]``."""
     if not _on_fabric():
         return dist.reduce_scatter(output, input_list, op=op, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("reduce_scatter")
     name = reduce_op_name(op)
-    if len(input_list) != _COMM.world:
-        raise ValueError(f"reduce_scatter: input_list has {len(input_list)} tensors, world size is {_COMM.world}")
+    if len(input_list) != comm.world:
+        raise ValueError(f"reduce_scatter: input_list has {len(input_list)} tensors, world size is {comm.world}")
     for t in input_list:
         if t.dtype != output.dtype or t.numel() != output.numel():
             raise ValueError(f"reduce_scatter: every tensor of input_list must be {output.dtype} with {output.numel()} elements")
-    _COMM.reduce_scatter_(output, torch.cat([t.reshape(-1) for t in input_list]), name)
+    comm.reduce_scatter_(output, torch.cat([t.reshape(-1) for t in input_list]), name)
     return None
 
 
-def broadcast(tensor: torch.Tensor, src: int, group: Any = None, async_op: bool = False) -> Any:
+def broadcast(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, async_op: bool = False,
+              group_src: Optional[int] = None) -> Any:
     """``torch.distributed.broadcast`` in place: every rank's ``tensor`` <- rank ``src``'s, bit for bit."""
     if not _on_fabric():
-        return dist.broadcast(tensor, src, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.broadcast_(tensor, root=src)
+        return dist.broadcast(tensor, src, group=group, async_op=async_op, **_given(group_src=group_src))
+    comm = _comm_for(group, async_op)
+    if _is_group(group):
+        root = _group_rank("broadcast", "src", group, src, group_src)
+        if comm is None:
+            return _not_in_group("broadcast")
+    else:
+        root = _world_rank(src, group_src)
+    comm.broadcast_(tensor, root=root)
     return None
 
 
@@ -250,8 +458,11 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     if not _on_fabric():
         return dist.all_to_all_single(output, input, output_split_sizes=output_split_sizes, input_split_sizes=input_split_sizes,
                                       group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.alltoall_(_split_rows(output, output_split_sizes, "output"), _split_rows(input, input_split_sizes, "input"))
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("all_to_all_single")
+    comm.alltoall_(_split_rows(output, output_split_sizes, "output", comm.world),
+                   _split_rows(input, input_split_sizes, "input", comm.world))
     return None
 
 
@@ -261,31 +472,48 @@ def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[t
     ``init_pg("b200")`` the tensors are used where they are (contiguous, one dtype), with no packing copy."""
     if not _on_fabric():
         return dist.all_to_all(output_tensor_list, input_tensor_list, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    _COMM.alltoall_(output_tensor_list, input_tensor_list)
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("all_to_all")
+    comm.alltoall_(output_tensor_list, input_tensor_list)
     return None
 
 
-def send(tensor: torch.Tensor, dst: int, group: Any = None, tag: int = 0) -> None:
+def send(tensor: torch.Tensor, dst: Optional[int] = None, group: Any = None, tag: int = 0,
+         group_dst: Optional[int] = None) -> None:
     """``torch.distributed.send``: rank ``dst`` receives ``tensor``'s bytes.  Under ``init_pg("b200")`` it is enqueued on the
     current stream (as NCCL's is) and messages to one rank match that rank's receives in issue order; ``tag`` is accepted
     and ignored, as torch's NCCL backend does."""
     if not _on_fabric():
-        return dist.send(tensor, dst, group=group, tag=tag)
-    _check_native_call(group, False)
-    _COMM.p2p_([("send", tensor, dst)])
+        return dist.send(tensor, dst, group=group, tag=tag, **_given(group_dst=group_dst))
+    comm = _comm_for(group)
+    if _is_group(group):
+        peer = _group_rank("send", "dst", group, dst, group_dst, default=None)
+        if comm is None:
+            return _not_in_group("send")
+    else:
+        peer = _world_rank(dst, group_dst)
+    comm.p2p_([("send", tensor, peer)])
     return None
 
 
-def recv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0) -> int:
+def recv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0,
+         group_src: Optional[int] = None) -> int:
     """``torch.distributed.recv``: ``tensor`` <- the next message rank ``src`` sends this rank (it must have as many bytes);
-    returns ``src``.  Receiving from any rank (``src=None``) is not available on the fabric."""
+    returns ``src`` (the global rank).  Receiving from any rank (``src=None``) is not available on the fabric."""
     if not _on_fabric():
-        return dist.recv(tensor, src, group=group, tag=tag)
-    _check_native_call(group, False)
-    if src is None:
+        return dist.recv(tensor, src, group=group, tag=tag, **_given(group_src=group_src))
+    comm = _comm_for(group)
+    if comm is None:
+        return _not_in_group("irecv", -1)
+    if src is None and group_src is None:
         raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    _COMM.p2p_([("recv", tensor, src)])
+    if _is_group(group):
+        peer = _group_rank("recv", "src", group, src, group_src)
+        comm.p2p_([("recv", tensor, peer)])
+        return group.get_global_rank(peer)
+    src = _world_rank(src, group_src)
+    comm.p2p_([("recv", tensor, src)])
     return src
 
 
@@ -304,52 +532,77 @@ class _P2PWork:
         return self._event.query()
 
 
-def _p2p_batch(ops: List[Any]) -> _P2PWork:
-    _COMM.p2p_(ops)
+def _p2p_batch(ops: List[Any], comm: Any = None) -> _P2PWork:
+    comm = _COMM if comm is None else comm
+    comm.p2p_(ops)
     event = torch.cuda.Event()
-    event.record(torch.cuda.current_stream(_COMM.device))
+    event.record(torch.cuda.current_stream(comm.device))
     return _P2PWork(event)
 
 
-def isend(tensor: torch.Tensor, dst: int, group: Any = None, tag: int = 0) -> Any:
+def isend(tensor: torch.Tensor, dst: Optional[int] = None, group: Any = None, tag: int = 0,
+          group_dst: Optional[int] = None) -> Any:
     """``torch.distributed.isend``: ``send`` returning a work handle."""
     if not _on_fabric():
-        return dist.isend(tensor, dst, group=group, tag=tag)
-    _check_native_call(group, False)
-    return _p2p_batch([("send", tensor, dst)])
+        return dist.isend(tensor, dst, group=group, tag=tag, **_given(group_dst=group_dst))
+    comm = _comm_for(group)
+    if _is_group(group):
+        peer = _group_rank("isend", "dst", group, dst, group_dst, default=None)
+        if comm is None:
+            return _not_in_group("isend")
+    else:
+        peer = _world_rank(dst, group_dst)
+    return _p2p_batch([("send", tensor, peer)], comm)
 
 
-def irecv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0) -> Any:
+def irecv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag: int = 0,
+          group_src: Optional[int] = None) -> Any:
     """``torch.distributed.irecv``: ``recv`` returning a work handle."""
     if not _on_fabric():
-        return dist.irecv(tensor, src, group=group, tag=tag)
-    _check_native_call(group, False)
-    if src is None:
+        return dist.irecv(tensor, src, group=group, tag=tag, **_given(group_src=group_src))
+    comm = _comm_for(group)
+    if comm is None:
+        return _not_in_group("irecv")
+    if src is None and group_src is None:
         raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    return _p2p_batch([("recv", tensor, src)])
+    if _is_group(group):
+        peer = _group_rank("irecv", "src", group, src, group_src)
+    else:
+        peer = _world_rank(src, group_src)
+    return _p2p_batch([("recv", tensor, peer)], comm)
 
 
 class P2POp:
     """``torch.distributed.P2POp``: one entry of ``batch_isend_irecv``.  ``op`` is ``isend`` or ``irecv`` (this module's or
     torch.distributed's).  Under ``init_pg("b200")`` it is a plain record, so it needs no process group; with one it is
     ``torch.distributed.P2POp`` itself, built with torch's ``isend`` / ``irecv`` in place of this module's, so a script
-    written with ``P2POp(isend, ...)`` runs under either backend."""
+    written with ``P2POp(isend, ...)`` runs under either backend.  With a ``B200Group``, ``peer`` is a global rank and
+    ``group_peer`` a rank of the group; the record keeps both."""
 
-    def __new__(cls, op: Any, tensor: torch.Tensor, peer: Optional[int] = None, group: Any = None, tag: int = 0) -> Any:
+    def __new__(cls, op: Any, tensor: torch.Tensor, peer: Optional[int] = None, group: Any = None, tag: int = 0,
+                group_peer: Optional[int] = None) -> Any:
         if not _on_fabric():
             op = dist.isend if op is isend else (dist.irecv if op is irecv else op)
-            return dist.P2POp(op, tensor, peer, group, tag)
+            return dist.P2POp(op, tensor, peer, group, tag, **_given(group_peer=group_peer))
         if op not in (isend, irecv, dist.isend, dist.irecv):
             raise ValueError("Invalid ``op``. Expected ``op`` to be of type ``torch.distributed.isend`` or ``torch.distributed.irecv``.")
         self = super().__new__(cls)
-        self.op, self.tensor, self.peer, self.group, self.tag = op, tensor, peer, group, tag
+        self.op, self.tensor, self.group, self.tag = op, tensor, group, tag
+        if _is_group(group):
+            if _is_non_member(group):  # torch translates the peer at construction, which a non-member cannot
+                raise ValueError("P2POp: this rank is not a member of the group, so its peer cannot be translated")
+            self.group_peer = _group_rank("P2POp", "peer", group, peer, group_peer, default=None)
+            self.peer = group.get_global_rank(self.group_peer)
+        else:
+            self.peer = _world_rank(peer, group_peer)
+            self.group_peer = self.peer
         return self
 
 
 def batch_isend_irecv(p2p_op_list: List[Any]) -> List[Any]:
     """``torch.distributed.batch_isend_irecv``: every op of the list in ONE launch under ``init_pg("b200")``, one handle per
     op.  A list longer than the fabric's 64 ops is refused rather than split: the ops of one launch cannot wait on each
-    other, and split launches could."""
+    other, and split launches could.  All ops name one group, as torch requires."""
     if not _on_fabric():
         return dist.batch_isend_irecv(p2p_op_list)
     from torchx_b200.ddp._native import B2_P2P_MAX_OPS
@@ -359,66 +612,89 @@ def batch_isend_irecv(p2p_op_list: List[Any]) -> List[Any]:
     if len(p2p_op_list) > B2_P2P_MAX_OPS:
         raise ValueError(f"batch_isend_irecv: {len(p2p_op_list)} ops, the b200 communicator takes at most {B2_P2P_MAX_OPS} "
                          "in one batch")
+    group = p2p_op_list[0].group
     ops = []
     for p in p2p_op_list:
-        _check_native_call(p.group, False)
-        if p.peer is None:
+        if _is_group(group) or _is_group(p.group):
+            if p.group is not group:
+                raise ValueError("All ops need to use the same group.")
+            comm = _comm_for(group)
+            peer = p.group_peer
+        else:
+            _check_native_call(p.group, False)
+            comm = _COMM
+            peer = p.peer
+        if peer is None:
             raise NotImplementedError("the b200 communicator cannot receive from any source: pass peer")
-        ops.append(("send" if p.op in (isend, dist.isend) else "recv", p.tensor, p.peer))
-    work = _p2p_batch(ops)
+        ops.append(("send" if p.op in (isend, dist.isend) else "recv", p.tensor, peer))
+    work = _p2p_batch(ops, comm)
     return [work] * len(ops)
 
 
-def _check_rank(name: str, r: Any) -> int:
+def _check_rank(name: str, r: Any, world: Optional[int] = None) -> int:
     from torchx_b200.ddp.comm import as_rank
 
+    world = _COMM.world if world is None else world
     k = as_rank(r)
-    if k is None or not 0 <= k < _COMM.world:
-        raise ValueError(f"{name} {r!r} is not a rank of a world of {_COMM.world}")
+    if k is None or not 0 <= k < world:
+        raise ValueError(f"{name} {r!r} is not a rank of a world of {world}")
     return k
 
 
-def gather(tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]] = None, dst: int = 0, group: Any = None,
-           async_op: bool = False) -> Any:
-    """``torch.distributed.gather``: on rank ``dst``, ``gather_list[r]`` <- rank r's ``tensor``.  Under ``init_pg("b200")``
-    rank ``dst`` runs one batch of W - 1 receives and copies its own tensor; every other rank runs one send."""
+def gather(tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]] = None, dst: Optional[int] = None, group: Any = None,
+           async_op: bool = False, group_dst: Optional[int] = None) -> Any:
+    """``torch.distributed.gather``: on rank ``dst`` (default 0), ``gather_list[r]`` <- rank r's ``tensor``.  Under
+    ``init_pg("b200")`` rank ``dst`` runs one batch of W - 1 receives and copies its own tensor; every other rank runs one
+    send."""
     if not _on_fabric():
-        return dist.gather(tensor, gather_list, dst=dst, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    dst = _check_rank("gather: dst", dst)
-    if _COMM.rank != dst:
+        return dist.gather(tensor, gather_list, dst=0 if dst is None and group_dst is None else dst, group=group, async_op=async_op,
+                           **_given(group_dst=group_dst))
+    comm = _comm_for(group, async_op)
+    if comm is None:
+        return _not_in_group("gather")
+    if _is_group(group):
+        dst = _group_rank("gather", "dst", group, dst, group_dst)
+    else:
+        dst = _check_rank("gather: dst", _world_rank(0 if dst is None and group_dst is None else dst, group_dst))
+    if comm.rank != dst:
         if gather_list:
             raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
-        _COMM.p2p_([("send", tensor, dst)])
+        comm.p2p_([("send", tensor, dst)])
         return None
     if not gather_list:
         raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
-    _check_list("gather: gather_list", gather_list, tensor)
-    if _COMM.world > 1:
-        _COMM.p2p_([("recv", t, r) for r, t in enumerate(gather_list) if r != dst])
+    _check_list("gather: gather_list", gather_list, tensor, comm.world)
+    if comm.world > 1:
+        comm.p2p_([("recv", t, r) for r, t in enumerate(gather_list) if r != dst])
     gather_list[dst].copy_(tensor)
     return None
 
 
-def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = None, src: int = 0, group: Any = None,
-            async_op: bool = False) -> Any:
-    """``torch.distributed.scatter``: every rank r's ``tensor`` <- ``scatter_list[r]`` of rank ``src``.  Under
+def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = None, src: Optional[int] = None, group: Any = None,
+            async_op: bool = False, group_src: Optional[int] = None) -> Any:
+    """``torch.distributed.scatter``: every rank r's ``tensor`` <- ``scatter_list[r]`` of rank ``src`` (default 0).  Under
     ``init_pg("b200")`` rank ``src`` runs one batch of W - 1 sends and copies its own block; every other rank runs one
     receive."""
     if not _on_fabric():
-        return dist.scatter(tensor, scatter_list, src=src, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    src = _check_rank("scatter: src", src)
-    if _COMM.rank != src:
+        return dist.scatter(tensor, scatter_list, src=0 if src is None and group_src is None else src, group=group,
+                            async_op=async_op, **_given(group_src=group_src))
+    comm = _comm_for(group, async_op)
+    if _is_group(group):
+        src = _group_rank("scatter", "src", group, src, group_src)
+        if comm is None:
+            return _not_in_group("scatter")
+    else:
+        src = _check_rank("scatter: src", _world_rank(0 if src is None and group_src is None else src, group_src))
+    if comm.rank != src:
         if scatter_list:
             raise ValueError("Argument ``scatter_list`` must NOT be specified on non-source ranks.")
-        _COMM.p2p_([("recv", tensor, src)])
+        comm.p2p_([("recv", tensor, src)])
         return None
     if not scatter_list:
         raise ValueError("Argument ``scatter_list`` must be specified on source rank.")
-    _check_list("scatter: scatter_list", scatter_list, tensor)
-    if _COMM.world > 1:
-        _COMM.p2p_([("send", t, r) for r, t in enumerate(scatter_list) if r != src])
+    _check_list("scatter: scatter_list", scatter_list, tensor, comm.world)
+    if comm.world > 1:
+        comm.p2p_([("send", t, r) for r, t in enumerate(scatter_list) if r != src])
     tensor.copy_(scatter_list[src])
     return None
 
@@ -432,15 +708,21 @@ def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor, worl
             raise ValueError(f"{what}: every tensor must be {like.dtype} with {like.numel()} elements")
 
 
-def reduce(tensor: torch.Tensor, dst: int, op: Any = dist.ReduceOp.SUM, group: Any = None, async_op: bool = False) -> Any:
+def reduce(tensor: torch.Tensor, dst: Optional[int] = None, op: Any = dist.ReduceOp.SUM, group: Any = None,
+           async_op: bool = False, group_dst: Optional[int] = None) -> Any:
     """``torch.distributed.reduce`` in place: on rank ``dst``, ``tensor`` <- the reduction over ranks of ``tensor``; every
     other rank's ``tensor`` is only read.  Under ``init_pg("b200")`` rank ``dst`` ends with the bits ``all_reduce`` with the
     same op leaves (include/b200ddp.h: b2_reduce), and each rank sends (W-1)/W of the tensor."""
     if not _on_fabric():
-        return dist.reduce(tensor, dst, op=op, group=group, async_op=async_op)
-    _check_native_call(group, async_op)
-    dst = _check_rank("reduce: dst", dst)
-    _COMM.reduce_(tensor, dst, reduce_op_name(op))
+        return dist.reduce(tensor, dst, op=op, group=group, async_op=async_op, **_given(group_dst=group_dst))
+    comm = _comm_for(group, async_op)
+    if _is_group(group):
+        dst = _group_rank("reduce", "dst", group, dst, group_dst, default=None)
+        if comm is None:
+            return _not_in_group("reduce")
+    else:
+        dst = _check_rank("reduce: dst", _world_rank(dst, group_dst))
+    comm.reduce_(tensor, dst, reduce_op_name(op))
     return None
 
 
@@ -456,9 +738,10 @@ def _comm_device() -> torch.device:
 
 
 def _check_object_call(fn: str, group: Any, device: Any = None) -> torch.device:
-    """The device an object collective runs on: the communicator's.  ``group`` must be None or WORLD and ``device``, if
-    given, the communicator's device: the fabric never moves the exchange elsewhere."""
-    _check_native_call(group, False)
+    """The device an object collective runs on: the communicator's.  ``group`` must be None, WORLD or a ``B200Group`` (or
+    ``NON_GROUP_MEMBER``) and ``device``, if given, the communicator's device: the fabric never moves the exchange
+    elsewhere."""
+    _comm_for(group)
     here = _comm_device()
     if device is not None:
         d = torch.device(device)
@@ -469,9 +752,11 @@ def _check_object_call(fn: str, group: Any, device: Any = None) -> torch.device:
     return here
 
 
-def _peer_arg(fn: str, name: str, r: Any, group_r: Any, default: Optional[int] = 0) -> int:
-    """``src`` / ``dst`` of an object collective; ``group_src`` / ``group_dst`` may stand in for it or repeat it (with no
-    subgroups the group rank is the rank)."""
+def _peer_arg(fn: str, name: str, r: Any, group_r: Any, default: Optional[int] = 0, group: Any = None) -> int:
+    """``src`` / ``dst`` of an object collective, as a rank of ``group``'s communicator.  On the world ``group_src`` /
+    ``group_dst`` may stand in for it or repeat it (the world's group rank is the rank); on a group see ``_group_rank``."""
+    if _is_group(group):
+        return _group_rank(fn, name, group, r, group_r, default)
     if group_r is not None:
         if r is not None and r != group_r:
             raise ValueError(f"{fn}: group_{name} {group_r!r} differs from {name} {r!r}; the b200 communicator has no subgroups")
@@ -513,14 +798,17 @@ def all_gather_object(object_list: List[Any], obj: Any, group: Any = None) -> No
     if not _on_fabric():
         return dist.all_gather_object(object_list, obj, group=group)
     device = _check_object_call("all_gather_object", group)
-    W = _COMM.world
+    comm = _comm_for(group)
+    if comm is None:
+        return _not_in_group("all_gather_object")
+    W = comm.world
     mine = _to_bytes(obj, device)
     sizes = torch.empty(W, dtype=torch.int64, device=device)
-    _COMM.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
+    comm.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
     sizes = sizes.tolist()
     block = max(sizes)
     out = torch.empty(W * block, dtype=torch.uint8, device=device)
-    _COMM.allgather_(out, _padded(mine, block))
+    comm.allgather_(out, _padded(mine, block))
     host = out.cpu().numpy().tobytes()
     for r in range(W):
         object_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
@@ -535,22 +823,26 @@ def gather_object(obj: Any, object_gather_list: Optional[List[Any]] = None, dst:
     if not _on_fabric():
         return dist.gather_object(obj, object_gather_list, dst=dst, group=group, group_dst=group_dst)
     device = _check_object_call("gather_object", group)
-    dst = _peer_arg("gather_object", "dst", dst, group_dst)
-    if _COMM.rank == dst and not object_gather_list:
+    comm = _comm_for(group)
+    dst = _peer_arg("gather_object", "dst", dst, group_dst, group=group)
+    if comm is None:
+        return _not_in_group("gather_object")
+    if comm.rank == dst and not object_gather_list:
         raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
-    if _COMM.rank != dst and object_gather_list:
+    if comm.rank != dst and object_gather_list:
         raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
-    W = _COMM.world
+    W = comm.world
     mine = _to_bytes(obj, device)
     sizes = torch.empty(W, dtype=torch.int64, device=device)
-    _COMM.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
+    comm.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
     sizes = sizes.tolist()
     block = max(sizes)
-    if _COMM.rank != dst:
-        gather(_padded(mine, block), None, dst=dst)
+    grp = group if _is_group(group) else None
+    if comm.rank != dst:
+        gather(_padded(mine, block), None, group=grp, group_dst=dst)
         return None
     out = torch.empty(W, block, dtype=torch.uint8, device=device)
-    gather(_padded(mine, block), list(out.unbind(0)), dst=dst)
+    gather(_padded(mine, block), list(out.unbind(0)), group=grp, group_dst=dst)
     host = out.cpu().numpy().tobytes()
     for r in range(W):
         object_gather_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
@@ -565,17 +857,20 @@ def broadcast_object_list(object_list: List[Any], src: Optional[int] = None, gro
     if not _on_fabric():
         return dist.broadcast_object_list(object_list, src=src, group=group, device=device, group_src=group_src)
     dev = _check_object_call("broadcast_object_list", group, device)
-    src = _peer_arg("broadcast_object_list", "src", src, group_src)
-    if _COMM.rank == src:
+    comm = _comm_for(group)
+    src = _peer_arg("broadcast_object_list", "src", src, group_src, group=group)
+    if comm is None:
+        return _not_in_group("broadcast_object_list")
+    if comm.rank == src:
         sizes, data = _concat_sizes([_to_bytes(o, dev) for o in object_list], dev)
-        _COMM.broadcast_(sizes, root=src)
-        _COMM.broadcast_(data, root=src)
+        comm.broadcast_(sizes, root=src)
+        comm.broadcast_(data, root=src)
         return None
     sizes = torch.empty(len(object_list), dtype=torch.int64, device=dev)
-    _COMM.broadcast_(sizes, root=src)
+    comm.broadcast_(sizes, root=src)
     sizes = sizes.tolist()
     data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
-    _COMM.broadcast_(data, root=src)
+    comm.broadcast_(data, root=src)
     _split_objects(object_list, sizes, data)
     return None
 
@@ -589,29 +884,33 @@ def scatter_object_list(scatter_object_output_list: List[Any], scatter_object_in
         return dist.scatter_object_list(scatter_object_output_list, scatter_object_input_list, src=src, group=group,
                                         group_src=group_src)
     device = _check_object_call("scatter_object_list", group)
-    src = _peer_arg("scatter_object_list", "src", src, group_src)
+    comm = _comm_for(group)
+    src = _peer_arg("scatter_object_list", "src", src, group_src, group=group)
+    if comm is None:
+        return _not_in_group("scatter_object_list")
     if not isinstance(scatter_object_output_list, list) or len(scatter_object_output_list) < 1:
         raise ValueError("Expected argument scatter_object_output_list to be a list of size at least 1.")
-    W = _COMM.world
-    if _COMM.rank == src:
+    W = comm.world
+    grp = group if _is_group(group) else None
+    if comm.rank == src:
         if scatter_object_input_list is None:
             raise ValueError("source rank must provide non-None scatter_object_input_list")
         if len(scatter_object_input_list) != W:
             raise ValueError(f"scatter_object_list: scatter_object_input_list has {len(scatter_object_input_list)} objects, "
                              f"world size is {W}")
         parts = [_to_bytes(o, device) for o in scatter_object_input_list]
-        _COMM.broadcast_(torch.tensor([t.numel() for t in parts], dtype=torch.int64).to(device), root=src)
+        comm.broadcast_(torch.tensor([t.numel() for t in parts], dtype=torch.int64).to(device), root=src)
         block = max(t.numel() for t in parts)
         out = torch.empty(block, dtype=torch.uint8, device=device)
-        scatter(out, [_padded(t, block) for t in parts], src=src)
+        scatter(out, [_padded(t, block) for t in parts], group=grp, group_src=src)
         n = parts[src].numel()
     else:
         sizes = torch.empty(W, dtype=torch.int64, device=device)
-        _COMM.broadcast_(sizes, root=src)
+        comm.broadcast_(sizes, root=src)
         sizes = sizes.tolist()
         out = torch.empty(max(sizes), dtype=torch.uint8, device=device)
-        scatter(out, None, src=src)
-        n = sizes[_COMM.rank]
+        scatter(out, None, group=grp, group_src=src)
+        n = sizes[comm.rank]
     scatter_object_output_list[0] = pickle.loads(out[:n].cpu().numpy().tobytes())
     return None
 
@@ -623,31 +922,37 @@ def send_object_list(object_list: List[Any], dst: Optional[int] = None, group: A
     if not _on_fabric():
         return dist.send_object_list(object_list, dst=dst, group=group, device=device, group_dst=group_dst, use_batch=use_batch)
     dev = _check_object_call("send_object_list", group, device)
-    dst = _peer_arg("send_object_list", "dst", dst, group_dst, default=None)
+    comm = _comm_for(group)
+    dst = _peer_arg("send_object_list", "dst", dst, group_dst, default=None, group=group)
+    if comm is None:
+        return _not_in_group("send_object_list")
     sizes, data = _concat_sizes([_to_bytes(o, dev) for o in object_list], dev)
-    _COMM.p2p_([("send", sizes, dst)])
-    _COMM.p2p_([("send", data, dst)])
+    comm.p2p_([("send", sizes, dst)])
+    comm.p2p_([("send", data, dst)])
     return None
 
 
 def recv_object_list(object_list: List[Any], src: Optional[int] = None, group: Any = None, device: Any = None,
                      group_src: Optional[int] = None, use_batch: bool = False) -> int:
     """``torch.distributed.recv_object_list``: ``object_list`` (as long as the sender's) <- the objects rank ``src`` sends
-    with ``send_object_list``, in place; returns ``src``.  Receiving from any rank is not available on the fabric.
-    Unpickling trusts rank ``src``."""
+    with ``send_object_list``, in place; returns ``src`` (the global rank).  Receiving from any rank is not available on the
+    fabric.  Unpickling trusts rank ``src``."""
     if not _on_fabric():
         return dist.recv_object_list(object_list, src=src, group=group, device=device, group_src=group_src, use_batch=use_batch)
     dev = _check_object_call("recv_object_list", group, device)
+    comm = _comm_for(group)
     if src is None and group_src is None:
         raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    src = _peer_arg("recv_object_list", "src", src, group_src)
+    src = _peer_arg("recv_object_list", "src", src, group_src, group=group)
+    if comm is None:
+        return _not_in_group("recv_object_list", -1)
     sizes = torch.empty(len(object_list), dtype=torch.int64, device=dev)
-    _COMM.p2p_([("recv", sizes, src)])
+    comm.p2p_([("recv", sizes, src)])
     sizes = sizes.tolist()
     data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
-    _COMM.p2p_([("recv", data, src)])
+    comm.p2p_([("recv", data, src)])
     _split_objects(object_list, sizes, data)
-    return src
+    return group.get_global_rank(src) if isinstance(group, B200Group) else src
 
 
 @contextmanager

@@ -98,8 +98,9 @@ class SyncBatchNorm(nn.SyncBatchNorm):
     On the fabric (``init_pg("b200")`` and no process group), in training with batch statistics and more than one rank,
     the forward's statistics and the backward's gradient sums are exchanged on the native communicator; the result is
     the same bits as torch's SyncBatchNorm forward (DESIGN.md 2.4).  In eval mode or at one rank it falls back to
-    ``F.batch_norm`` as torch does.  Off the fabric it is torch's module.  Refused on the fabric: a ``process_group``
-    other than the whole world (NotImplementedError), running statistics that are not float32 (TypeError) and a CPU
+    ``F.batch_norm`` as torch does.  Off the fabric it is torch's module.  With ``process_group`` a ``B200Group``
+    (``torchx_b200.distributed.new_group``) the layer synchronises over the group's ranks only.  Refused on the fabric: any
+    other ``process_group`` but the whole world (NotImplementedError), running statistics that are not float32 (TypeError) and a CPU
     input (ValueError)."""
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:  # noqa: A002
@@ -123,8 +124,11 @@ class SyncBatchNorm(nn.SyncBatchNorm):
         comm = _dist.communicator()
         need_sync = bn_training and self.training
         if need_sync:
-            if self.process_group is not None and self.process_group is not dist.group.WORLD:
-                raise NotImplementedError("the b200 communicator has no subgroups: SyncBatchNorm needs process_group=None")
+            if isinstance(self.process_group, _dist.B200Group):
+                comm = self.process_group.comm  # the statistics of the group's ranks only, merged in group-rank order
+            elif self.process_group is not None and self.process_group is not dist.group.WORLD:
+                raise NotImplementedError("the b200 communicator has no subgroups but a B200Group: SyncBatchNorm needs "
+                                          "process_group=None or a torchx_b200.distributed.new_group group")
             for name, t in (("running_mean", running_mean), ("running_var", running_var)):
                 if t is not None and t.dtype != torch.float32:
                     raise TypeError(f"SyncBatchNorm on the b200 communicator keeps float32 running statistics, {name} is {t.dtype}")
