@@ -151,6 +151,31 @@ def test_creator_takes_the_communicator_from_the_environment(monkeypatch):
     assert D._COMM is fake
 
 
+@pytest.mark.parametrize("first", ["init_pg", "init_process_group", "mini_ddp", "hook_state"])
+def test_every_entry_point_shares_one_process_communicator(monkeypatch, first):
+    """Whichever entry point comes first makes the communicator from the environment; the others reuse it."""
+    from torchx_b200.ddp import B200HookState, DistributedDataParallel
+
+    fake, made = _FakeComm(0, 1), []
+    monkeypatch.setattr(D, "_COMM", None)
+    monkeypatch.setattr(Communicator, "from_env", classmethod(lambda cls, **kw: made.append(kw) or fake))
+    monkeypatch.setattr(torch.cuda, "Stream", lambda device=None: None)
+    monkeypatch.setattr(torch.cuda, "Event", lambda: None)
+
+    def mini_ddp():
+        with pytest.raises(ValueError, match="parameter on cpu, communicator on cuda:0"):  # after it took the communicator
+            DistributedDataParallel(torch.nn.Linear(2, 2))
+
+    entries = {"init_pg": lambda: D.init_pg("b200"), "init_process_group": lambda: B._create(_Opts(0, 1, [])),
+               "mini_ddp": mini_ddp, "hook_state": lambda: B200HookState()}
+    entries.pop(first)()
+    assert D._COMM is fake and made == [{}]
+    for enter in entries.values():
+        enter()
+    assert D.init_pg("b200") == torch.device("cuda", 0) and B200HookState().comm is fake
+    assert B._create(_Opts(0, 1, [])).comm is fake and made == [{}]
+
+
 def test_the_group_installs_no_stream_over_an_owner():
     fake = _FakeComm(0, 2)
     owner = fake.ordered_stream

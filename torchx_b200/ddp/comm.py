@@ -69,6 +69,47 @@ def as_rank(x) -> Optional[int]:
         return None
 
 
+# ---- checks shared with the "b200" process group, which makes them before it enqueues anything -----------------------
+def check_allgather(comm, out: torch.Tensor, t: torch.Tensor) -> None:
+    """``allgather_``'s checks: ``out`` has ``t``'s dtype and world x its size, both tensors on ``comm``'s device."""
+    if out.dtype != t.dtype:
+        raise TypeError(f"allgather_: out is {out.dtype}, input is {t.dtype}")
+    comm._check_tensor(out)
+    comm._check_tensor(t)
+    if out.numel() != comm.world * t.numel():
+        raise ValueError(f"allgather_: out has {out.numel()} elements, needs {comm.world} x {t.numel()}")
+
+
+def check_reduce_scatter(comm, out: torch.Tensor, t: torch.Tensor, op: str):
+    """``reduce_scatter_``'s checks: the dtype and op, ``t`` of ``out``'s dtype and world x its size, both tensors on
+    ``comm``'s device.  Returns (B2_DT_*, B2_OP_*)."""
+    dt, code = dtype_op_for(t.dtype, op, "reduce_scatter_")
+    if out.dtype != t.dtype:
+        raise TypeError(f"reduce_scatter_: out is {out.dtype}, input is {t.dtype}")
+    if t.numel() != comm.world * out.numel():
+        raise ValueError(f"reduce_scatter_: input has {t.numel()} elements, needs {comm.world} x {out.numel()}")
+    comm._check_tensor(out)
+    comm._check_tensor(t)
+    return dt, code
+
+
+def check_alltoall(world: int, outs: Sequence[torch.Tensor], ins: Sequence[torch.Tensor]) -> None:
+    """``alltoall_``'s list checks: world tensors each way, all of one dtype."""
+    if len(outs) != world or len(ins) != world:
+        raise ValueError(f"alltoall_: needs {world} output and {world} input tensors, got {len(outs)} and {len(ins)}")
+    dtypes = {t.dtype for t in (*outs, *ins)}
+    if len(dtypes) > 1:
+        raise TypeError(f"alltoall_: every tensor must have one dtype, got {sorted(str(d) for d in dtypes)}")
+
+
+def check_peer(k: int, peer, rank: int, world: int) -> int:
+    """The peer of op ``k`` of a ``p2p_`` batch as an int: another rank of the world."""
+    p = as_rank(peer)
+    if p is None or not 0 <= p < world or p == rank:
+        raise ValueError(f"p2p_: op {k} names peer {peer!r}; rank {rank} of {world} can only name another rank")
+    return p
+
+
 def _stream_arg(stream: Optional[torch.cuda.Stream], device: int) -> ctypes.c_void_p:
     """The cudaStream_t argument of a library call: ``stream``, or the device's current stream."""
     s = stream if stream is not None else torch.cuda.current_stream(device)
@@ -270,12 +311,7 @@ class Communicator:
     def allgather_(self, out: torch.Tensor, t: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
         """``out`` (world x the size of ``t``, same dtype) <- every rank's ``t`` in rank order (b2_allgather).  ``t`` may be
         this rank's block of ``out``."""
-        if out.dtype != t.dtype:
-            raise TypeError(f"allgather_: out is {out.dtype}, input is {t.dtype}")
-        self._check_tensor(out)
-        self._check_tensor(t)
-        if out.numel() != self.world * t.numel():
-            raise ValueError(f"allgather_: out has {out.numel()} elements, needs {self.world} x {t.numel()}")
+        check_allgather(self, out, t)
         N.check(N.lib().b2_allgather(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()),
                                      t.numel() * t.element_size(), _stream_arg(stream, self.device)))
         return out
@@ -285,13 +321,7 @@ class Communicator:
         """``out`` <- block ``rank`` of the ``allreduce_op_`` of ``t`` (world x the size of ``out``, same dtype) over the ranks
         (include/b200ddp.h: b2_reduce_scatter): the same bits that allreduce leaves there, moving only (W-1)/W of ``t``.
         ``out`` may be this rank's block of ``t``."""
-        dt, code = dtype_op_for(t.dtype, op, "reduce_scatter_")
-        if out.dtype != t.dtype:
-            raise TypeError(f"reduce_scatter_: out is {out.dtype}, input is {t.dtype}")
-        if t.numel() != self.world * out.numel():
-            raise ValueError(f"reduce_scatter_: input has {t.numel()} elements, needs {self.world} x {out.numel()}")
-        self._check_tensor(out)
-        self._check_tensor(t)
+        dt, code = check_reduce_scatter(self, out, t, op)
         N.check(N.lib().b2_reduce_scatter(self._h, ctypes.c_void_p(out.data_ptr()), ctypes.c_void_p(t.data_ptr()), out.numel(), dt,
                                           code, _stream_arg(stream, self.device)))
         return out
@@ -351,11 +381,7 @@ class Communicator:
         contiguous tensors on this communicator's device, all of one dtype (any dtype: the copy is of bytes), of any sizes;
         ``outs[r]`` must have as many bytes as rank r sends this rank, and one pair of ranks carries at most
         ``alltoall_max_bytes``.  No tensor of ``outs`` may overlap another tensor of either list."""
-        if len(outs) != self.world or len(ins) != self.world:
-            raise ValueError(f"alltoall_: needs {self.world} output and {self.world} input tensors, got {len(outs)} and {len(ins)}")
-        dtypes = {t.dtype for t in (*outs, *ins)}
-        if len(dtypes) > 1:
-            raise TypeError(f"alltoall_: every tensor must have one dtype, got {sorted(str(d) for d in dtypes)}")
+        check_alltoall(self.world, outs, ins)
         for t in (*outs, *ins):
             self._check_tensor(t)
 
@@ -381,10 +407,7 @@ class Communicator:
         for k, (kind, _, peer) in enumerate(ops):
             if kind not in ("send", "recv"):
                 raise ValueError(f"p2p_: op {k} is {kind!r}, not 'send' or 'recv'")
-            p = as_rank(peer)
-            if p is None or not 0 <= p < self.world or p == self.rank:
-                raise ValueError(f"p2p_: op {k} names peer {peer!r}; rank {self.rank} of {self.world} can only name another rank")
-            peers.append(p)
+            peers.append(check_peer(k, peer, self.rank, self.world))
         arr = (N.B2P2pOp * len(ops))()
         for k, ((kind, t, _), peer) in enumerate(zip(ops, peers)):
             self._check_tensor(t)

@@ -163,11 +163,10 @@ class DistributedDataParallel(nn.Module):
     ) -> None:
         super().__init__()
         self.module = module
-        if comm is None:
-            # one communicator per process: reuse the one init_pg("b200") created (each one owns a 1 GiB arena)
-            from torchx_b200 import distributed as _dist
+        if comm is None:  # one communicator per process (each owns a multi-GiB arena)
+            from torchx_b200.distributed import process_communicator
 
-            comm = _dist._COMM if _dist._COMM is not None else Communicator.from_env()
+            comm = process_communicator()
         self.comm = comm
         self.world_size = self.comm.world
         self.wire = wire

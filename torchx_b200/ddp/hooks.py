@@ -20,10 +20,10 @@ from .comm import Communicator
 
 class B200HookState:
     def __init__(self, comm: Optional[Communicator] = None, wire: str = "bf16", algo: str = "auto") -> None:
-        if comm is None:  # one communicator per process: reuse the one init_pg("b200") created (each owns a multi-GiB arena)
-            from torchx_b200 import distributed as _dist
+        if comm is None:  # one communicator per process (each owns a multi-GiB arena)
+            from torchx_b200.distributed import process_communicator
 
-            comm = _dist._COMM if _dist._COMM is not None else Communicator.from_env()
+            comm = process_communicator()
         self.comm = comm
         self.wire = wire
         self.algo = algo

@@ -21,7 +21,7 @@ import os
 import pickle
 import warnings
 from contextlib import contextmanager
-from typing import Any, Iterator, List, Optional
+from typing import Any, Callable, Iterator, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -86,6 +86,18 @@ def communicator() -> Any:
     return _COMM
 
 
+def process_communicator(**kwargs: Any) -> Any:
+    """The process's one native communicator, ``_COMM``, made with ``Communicator.from_env(**kwargs)`` and stored if there
+    is none yet.  ``init_pg("b200")``, ``init_process_group("b200")``, the mini-DDP and ``B200HookState`` all take it from
+    here, so whichever comes first makes the communicator (and its multi-GiB arena) the others share."""
+    global _COMM
+    if _COMM is None:
+        from torchx_b200.ddp import Communicator
+
+        _COMM = Communicator.from_env(**kwargs)
+    return _COMM
+
+
 def is_torchelastic_launched() -> bool:
     return "TORCHELASTIC_RUN_ID" in os.environ
 
@@ -98,13 +110,8 @@ def init_pg(backend: str = "auto", **kwargs: Any) -> torch.device:
     As in the reference the caller selects the returned device (``torch.cuda.set_device`` / ``.to(device)``).
     ``b200``: rendezvous through the ``local_cuda`` scheduler's shm control block and CUDA IPC; no process group.
     """
-    global _COMM
     if backend == "b200":
-        if _COMM is None:
-            from torchx_b200.ddp import Communicator
-
-            _COMM = Communicator.from_env(**kwargs)
-        return torch.device("cuda", _COMM.device)
+        return torch.device("cuda", process_communicator(**kwargs).device)
     if backend == "auto":
         # a CUDA build of torch says is_available() on some CPU hosts: ask for actual devices and for NCCL itself
         has_gpu = torch.cuda.is_available() and torch.cuda.device_count() > 0 and dist.is_nccl_available()
@@ -121,7 +128,7 @@ def init_pg(backend: str = "auto", **kwargs: Any) -> torch.device:
 def barrier(group: Any = None) -> None:
     """A host-blocking barrier over the world, or over ``group`` (a ``B200Group``) under ``init_pg("b200")``."""
     if _COMM is not None and not dist.is_initialized():
-        comm = _comm_for(group)
+        comm, _ = _resolve("barrier", group)
         if comm is None:
             return _not_in_group("barrier")
         comm.barrier()
@@ -222,7 +229,7 @@ def new_subgroups_by_enumeration(ranks_per_subgroup_list: List[List[int]], timeo
     for ranks in ranks_per_subgroup_list:
         g = new_group(ranks)
         subgroups.append(g)
-        if isinstance(g, B200Group):
+        if not _is_non_member(g):
             cur = g
     return cur, subgroups
 
@@ -256,29 +263,65 @@ def new_subgroups(group_size: Optional[int] = None, group: Any = None, timeout: 
 
 _NO_SUBGROUPS = ("the b200 communicator has no subgroups but the B200Group of torchx_b200.distributed.new_group: pass "
                  "group=None or a B200Group")
+_NO_ANY_SOURCE = "the b200 communicator cannot receive from any source: pass src"
+_ANY_SOURCE = object()  # a _resolve default: a receive without src, which the fabric refuses
 
 
-def _comm_for(group: Any, async_op: bool = False) -> Any:
-    """The communicator a helper runs on: the world's for None / WORLD, the group's for a ``B200Group``, None for
-    ``NON_GROUP_MEMBER``.  Any other group, and ``async_op``, are refused."""
+def _resolve(fn: str, group: Any, async_op: bool = False, name: Optional[str] = None, r: Any = None, group_r: Any = None,
+             default: Any = 0, translate_first: bool = True, check: bool = True, world: Any = None) -> Tuple[Any, Any]:
+    """The communicator a helper runs on and, with ``name``, its root or peer as a rank of that communicator.
+
+    The communicator: ``world`` (default ``_COMM``) for ``group`` None / WORLD, the group's own for a ``B200Group``, None for
+    ``NON_GROUP_MEMBER``; any other group, and ``async_op``, are refused.  The root: ``r`` is the global rank the helper's
+    ``name`` argument gives, ``group_r`` its ``group_<name>``; with neither, ``default`` - a rank, None (refused below as
+    not a rank) or ``_ANY_SOURCE`` (refused).  On the world ``group_r`` may stand in for ``r`` or repeat it, and the root is
+    range-checked unless ``check`` is False (the communicator checks it).  On a group it is translated as torch's
+    ``_canonicalize_group_rank`` does: both given, or a rank outside the group, is a ValueError.  On ``NON_GROUP_MEMBER``
+    the root is translated first when ``translate_first`` (a global rank is then a ValueError, a group rank is returned
+    unchecked), else not at all: torch's helpers differ there."""
+    on_group = isinstance(group, B200Group)
     if group is None or group is dist.group.WORLD:
-        comm = _COMM
-    elif isinstance(group, B200Group):
-        comm = group.comm
-    elif _is_non_member(group):
-        comm = None
+        comm = _COMM if world is None else world
+    elif on_group or _is_non_member(group):
+        comm, on_group = group.comm if on_group else None, True
     else:
         raise NotImplementedError(_NO_SUBGROUPS)
     if async_op:
         raise NotImplementedError("the b200 communicator has no work handles: collectives are ordered on the current stream")
-    return comm
+    if name is None or (comm is None and not translate_first):
+        return comm, None
+    if on_group and r is not None and group_r is not None:
+        raise ValueError(f"{fn}: Can't specify both group_{name} ({group_r!r}) and {name} ({r!r})")
+    if not on_group and group_r is not None:
+        if r is not None and r != group_r:
+            raise ValueError(f"{fn}: group_{name} {group_r!r} differs from {name} {r!r}; the world's group ranks are its ranks")
+        r, group_r = group_r, None
+    if not on_group and not check:
+        return comm, r
+    if r is None and group_r is None:
+        if default is _ANY_SOURCE:
+            raise NotImplementedError(_NO_ANY_SOURCE)
+        r = default
+    from torchx_b200.ddp.comm import as_rank
+
+    if not on_group:
+        k = as_rank(r)
+        if k is None or not 0 <= k < comm.world:
+            raise ValueError(f"{fn}: {name} {r!r} is not a rank of a world of {comm.world}")
+        return comm, k
+    if group_r is not None:
+        k = as_rank(group_r)
+        if comm is not None and (k is None or not 0 <= k < comm.world):
+            raise ValueError(f"{fn}: group_{name} {group_r!r} is not a rank of a group of {comm.world}")
+        return comm, group_r if comm is None else k
+    if comm is None:
+        raise ValueError(f"{fn}: {name} {r!r} is a global rank, and this rank is not a member of the group to translate it")
+    return comm, group.get_group_rank(r)
 
 
-def _check_native_call(group: Any, async_op: bool) -> None:
-    if group is not None and group is not dist.group.WORLD:
-        raise NotImplementedError("the b200 communicator has no subgroups: pass group=None")
-    if async_op:
-        raise NotImplementedError("the b200 communicator has no work handles: collectives are ordered on the current stream")
+def _global_rank(group: Any, k: Any) -> Any:
+    """The global rank of rank ``k`` of the communicator ``_resolve`` returned for ``group``."""
+    return k if group is None or group is dist.group.WORLD else group.get_global_rank(k)
 
 
 def _not_in_group(op: str, ret: Any = None) -> Any:
@@ -287,46 +330,14 @@ def _not_in_group(op: str, ret: Any = None) -> Any:
     return ret
 
 
-def _group_rank(fn: str, name: str, group: Any, r: Any, group_r: Any, default: Optional[int] = 0) -> Any:
-    """The rank of ``group``'s communicator that a helper's ``name`` (a global rank) or ``group_name`` (a group rank)
-    names, as torch's ``_canonicalize_group_rank``: both given, a rank outside the group and, on ``NON_GROUP_MEMBER``, any
-    global rank are ValueErrors; on ``NON_GROUP_MEMBER`` a group rank is returned unchecked."""
-    if r is not None and group_r is not None:
-        raise ValueError(f"{fn}: Can't specify both group_{name} ({group_r!r}) and {name} ({r!r})")
-    if group_r is not None:
-        if _is_non_member(group):
-            return group_r
-        from torchx_b200.ddp.comm import as_rank
-
-        k = as_rank(group_r)
-        if k is None or not 0 <= k < group.comm.world:
-            raise ValueError(f"{fn}: group_{name} {group_r!r} is not a rank of a group of {group.comm.world}")
-        return k
-    if r is None:
-        if default is None:
-            raise ValueError(f"{fn}: {name} or group_{name} must be given")
-        r = default
-    if _is_non_member(group):
-        raise ValueError(f"{fn}: {name} {r!r} is a global rank, and this rank is not a member of the group to translate it")
-    return group.get_group_rank(r)
-
-
-def _world_rank(r: Any, group_r: Any) -> Any:
-    """``src`` / ``dst`` / ``peer`` on the world, where ``group_src`` ... is the same rank and may stand in for it."""
-    if group_r is None:
-        return r
-    if r is not None and r != group_r:
-        raise ValueError(f"group rank {group_r!r} differs from rank {r!r}; the world's group ranks are its ranks")
-    return group_r
-
-
 def _given(**kw: Any) -> dict:
     """The keyword arguments that were given: a call delegated to torch.distributed passes the group_* ranks only then."""
     return {k: v for k, v in kw.items() if v is not None}
 
 
-def _is_group(group: Any) -> bool:
-    return isinstance(group, B200Group) or _is_non_member(group)
+def _on(stream: Any) -> dict:
+    """The stream keyword of a Communicator call in a ``launch(stream)``: none for None, the current stream."""
+    return {} if stream is None else {"stream": stream}
 
 
 _REDUCE_OPS = ((dist.ReduceOp.SUM, "sum"), (dist.ReduceOp.AVG, "avg"), (dist.ReduceOp.MIN, "min"), (dist.ReduceOp.MAX, "max"))
@@ -346,7 +357,7 @@ def all_reduce(tensor: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = N
     With a process group it is ``torch.distributed.all_reduce``."""
     if not _on_fabric():
         return dist.all_reduce(tensor, op=op, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("all_reduce", group, async_op)
     if comm is None:
         return _not_in_group("all_reduce")
     comm.allreduce_op_(tensor, reduce_op_name(op))
@@ -359,7 +370,7 @@ def all_gather_into_tensor(output_tensor: torch.Tensor, input_tensor: torch.Tens
     along its first dimension (or, flat, as world consecutive blocks)."""
     if not _on_fabric():
         return dist.all_gather_into_tensor(output_tensor, input_tensor, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("all_gather_into_tensor", group, async_op)
     if comm is None:
         return _not_in_group("all_gather_into_tensor")
     comm.allgather_(output_tensor, input_tensor)
@@ -370,19 +381,25 @@ def all_gather(tensor_list: List[torch.Tensor], tensor: torch.Tensor, group: Any
     """``torch.distributed.all_gather``: ``tensor_list[r]`` <- rank r's ``tensor``."""
     if not _on_fabric():
         return dist.all_gather(tensor_list, tensor, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("all_gather", group, async_op)
     if comm is None:
         return _not_in_group("all_gather")
-    if len(tensor_list) != comm.world:
-        raise ValueError(f"all_gather: tensor_list has {len(tensor_list)} tensors, world size is {comm.world}")
-    for t in tensor_list:
-        if t.dtype != tensor.dtype or t.numel() != tensor.numel():
-            raise ValueError(f"all_gather: every tensor of tensor_list must be {tensor.dtype} with {tensor.numel()} elements")
-    flat = torch.empty((comm.world,) + tuple(tensor.shape), dtype=tensor.dtype, device=tensor.device)
-    comm.allgather_(flat, tensor.contiguous())
-    for r, t in enumerate(tensor_list):
-        t.copy_(flat[r].view_as(t))
+    _all_gather(comm, tensor_list, tensor.contiguous())(None)
     return None
+
+
+def _all_gather(comm: Any, tensor_list: List[torch.Tensor], tensor: torch.Tensor) -> Callable[[Any], None]:
+    """``all_gather``'s checks on ``comm``, and its ``launch(stream)``: one all-gather into a staging buffer, then a copy
+    per rank.  This and the list collectives below serve the helpers (``launch(None)``) and ``B200ProcessGroup``."""
+    _check_list("all_gather: tensor_list", tensor_list, tensor, comm.world, "all_gather: every tensor of tensor_list")
+
+    def launch(stream: Any) -> None:
+        flat = torch.empty((comm.world,) + tuple(tensor.shape), dtype=tensor.dtype, device=tensor.device)
+        comm.allgather_(flat, tensor, **_on(stream))
+        for r, t in enumerate(tensor_list):
+            t.copy_(flat[r].view_as(t))
+
+    return launch
 
 
 def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, op: Any = dist.ReduceOp.SUM, group: Any = None,
@@ -392,7 +409,7 @@ def reduce_scatter_tensor(output: torch.Tensor, input: torch.Tensor, op: Any = d
     block r of what ``all_reduce`` with the same op leaves, bit for bit, at (W-1)/W of the input's bytes per rank."""
     if not _on_fabric():
         return dist.reduce_scatter_tensor(output, input, op=op, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("reduce_scatter_tensor", group, async_op)
     if comm is None:
         return _not_in_group("reduce_scatter_tensor")
     comm.reduce_scatter_(output, input, reduce_op_name(op))
@@ -404,17 +421,17 @@ def reduce_scatter(output: torch.Tensor, input_list: List[torch.Tensor], op: Any
     """``torch.distributed.reduce_scatter``: rank r's ``output`` <- the reduction over ranks of their ``input_list[r]``."""
     if not _on_fabric():
         return dist.reduce_scatter(output, input_list, op=op, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("reduce_scatter", group, async_op)
     if comm is None:
         return _not_in_group("reduce_scatter")
-    name = reduce_op_name(op)
-    if len(input_list) != comm.world:
-        raise ValueError(f"reduce_scatter: input_list has {len(input_list)} tensors, world size is {comm.world}")
-    for t in input_list:
-        if t.dtype != output.dtype or t.numel() != output.numel():
-            raise ValueError(f"reduce_scatter: every tensor of input_list must be {output.dtype} with {output.numel()} elements")
-    comm.reduce_scatter_(output, torch.cat([t.reshape(-1) for t in input_list]), name)
+    _reduce_scatter(comm, output, input_list, reduce_op_name(op))(None)
     return None
+
+
+def _reduce_scatter(comm: Any, output: torch.Tensor, input_list: List[torch.Tensor], op: str) -> Callable[[Any], None]:
+    """``reduce_scatter``'s checks on ``comm``, and its ``launch(stream)``: the list concatenated, then one reduce-scatter."""
+    _check_list("reduce_scatter: input_list", input_list, output, comm.world, "reduce_scatter: every tensor of input_list")
+    return lambda stream: comm.reduce_scatter_(output, torch.cat([t.reshape(-1) for t in input_list]), op, **_on(stream))
 
 
 def broadcast(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, async_op: bool = False,
@@ -422,20 +439,15 @@ def broadcast(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None
     """``torch.distributed.broadcast`` in place: every rank's ``tensor`` <- rank ``src``'s, bit for bit."""
     if not _on_fabric():
         return dist.broadcast(tensor, src, group=group, async_op=async_op, **_given(group_src=group_src))
-    comm = _comm_for(group, async_op)
-    if _is_group(group):
-        root = _group_rank("broadcast", "src", group, src, group_src)
-        if comm is None:
-            return _not_in_group("broadcast")
-    else:
-        root = _world_rank(src, group_src)
+    comm, root = _resolve("broadcast", group, async_op, "src", src, group_src, check=False)
+    if comm is None:
+        return _not_in_group("broadcast")
     comm.broadcast_(tensor, root=root)
     return None
 
 
-def _split_rows(t: torch.Tensor, sizes: Optional[List[int]], what: str, world: Optional[int] = None) -> List[torch.Tensor]:
+def _split_rows(t: torch.Tensor, sizes: Optional[List[int]], what: str, world: int) -> List[torch.Tensor]:
     """``t`` cut along its first dimension into world views: ``sizes`` rows each, or evenly when ``sizes`` is None / empty."""
-    world = _COMM.world if world is None else world
     if not sizes:
         if t.size(0) % world:
             raise ValueError(f"all_to_all_single: {what} has {t.size(0)} rows, not a multiple of the world size {world}; "
@@ -458,12 +470,22 @@ def all_to_all_single(output: torch.Tensor, input: torch.Tensor, output_split_si
     if not _on_fabric():
         return dist.all_to_all_single(output, input, output_split_sizes=output_split_sizes, input_split_sizes=input_split_sizes,
                                       group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("all_to_all_single", group, async_op)
     if comm is None:
         return _not_in_group("all_to_all_single")
-    comm.alltoall_(_split_rows(output, output_split_sizes, "output", comm.world),
-                   _split_rows(input, input_split_sizes, "input", comm.world))
+    _all_to_all_single(comm, output, input, output_split_sizes, input_split_sizes)(None)
     return None
+
+
+def _all_to_all_single(comm: Any, output: torch.Tensor, input: torch.Tensor, output_split_sizes: Optional[List[int]],  # noqa: A002
+                       input_split_sizes: Optional[List[int]]) -> Callable[[Any], None]:
+    """``all_to_all_single``'s checks on ``comm``, and its ``launch(stream)``: one all-to-all between views of the two."""
+    from torchx_b200.ddp.comm import check_alltoall
+
+    outs = _split_rows(output, output_split_sizes, "output", comm.world)
+    ins = _split_rows(input, input_split_sizes, "input", comm.world)
+    check_alltoall(comm.world, outs, ins)
+    return lambda stream: comm.alltoall_(outs, ins, **_on(stream))
 
 
 def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[torch.Tensor], group: Any = None,
@@ -472,7 +494,7 @@ def all_to_all(output_tensor_list: List[torch.Tensor], input_tensor_list: List[t
     ``init_pg("b200")`` the tensors are used where they are (contiguous, one dtype), with no packing copy."""
     if not _on_fabric():
         return dist.all_to_all(output_tensor_list, input_tensor_list, group=group, async_op=async_op)
-    comm = _comm_for(group, async_op)
+    comm, _ = _resolve("all_to_all", group, async_op)
     if comm is None:
         return _not_in_group("all_to_all")
     comm.alltoall_(output_tensor_list, input_tensor_list)
@@ -486,13 +508,9 @@ def send(tensor: torch.Tensor, dst: Optional[int] = None, group: Any = None, tag
     and ignored, as torch's NCCL backend does."""
     if not _on_fabric():
         return dist.send(tensor, dst, group=group, tag=tag, **_given(group_dst=group_dst))
-    comm = _comm_for(group)
-    if _is_group(group):
-        peer = _group_rank("send", "dst", group, dst, group_dst, default=None)
-        if comm is None:
-            return _not_in_group("send")
-    else:
-        peer = _world_rank(dst, group_dst)
+    comm, peer = _resolve("send", group, False, "dst", dst, group_dst, default=None)
+    if comm is None:
+        return _not_in_group("send")
     comm.p2p_([("send", tensor, peer)])
     return None
 
@@ -503,18 +521,11 @@ def recv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, tag
     returns ``src`` (the global rank).  Receiving from any rank (``src=None``) is not available on the fabric."""
     if not _on_fabric():
         return dist.recv(tensor, src, group=group, tag=tag, **_given(group_src=group_src))
-    comm = _comm_for(group)
+    comm, peer = _resolve("recv", group, False, "src", src, group_src, default=_ANY_SOURCE, translate_first=False)
     if comm is None:
-        return _not_in_group("irecv", -1)
-    if src is None and group_src is None:
-        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    if _is_group(group):
-        peer = _group_rank("recv", "src", group, src, group_src)
-        comm.p2p_([("recv", tensor, peer)])
-        return group.get_global_rank(peer)
-    src = _world_rank(src, group_src)
-    comm.p2p_([("recv", tensor, src)])
-    return src
+        return _not_in_group("recv", -1)
+    comm.p2p_([("recv", tensor, peer)])
+    return _global_rank(group, peer)
 
 
 class _P2PWork:
@@ -532,8 +543,7 @@ class _P2PWork:
         return self._event.query()
 
 
-def _p2p_batch(ops: List[Any], comm: Any = None) -> _P2PWork:
-    comm = _COMM if comm is None else comm
+def _p2p_batch(ops: List[Any], comm: Any) -> _P2PWork:
     comm.p2p_(ops)
     event = torch.cuda.Event()
     event.record(torch.cuda.current_stream(comm.device))
@@ -545,13 +555,9 @@ def isend(tensor: torch.Tensor, dst: Optional[int] = None, group: Any = None, ta
     """``torch.distributed.isend``: ``send`` returning a work handle."""
     if not _on_fabric():
         return dist.isend(tensor, dst, group=group, tag=tag, **_given(group_dst=group_dst))
-    comm = _comm_for(group)
-    if _is_group(group):
-        peer = _group_rank("isend", "dst", group, dst, group_dst, default=None)
-        if comm is None:
-            return _not_in_group("isend")
-    else:
-        peer = _world_rank(dst, group_dst)
+    comm, peer = _resolve("isend", group, False, "dst", dst, group_dst, default=None)
+    if comm is None:
+        return _not_in_group("isend")
     return _p2p_batch([("send", tensor, peer)], comm)
 
 
@@ -560,15 +566,9 @@ def irecv(tensor: torch.Tensor, src: Optional[int] = None, group: Any = None, ta
     """``torch.distributed.irecv``: ``recv`` returning a work handle."""
     if not _on_fabric():
         return dist.irecv(tensor, src, group=group, tag=tag, **_given(group_src=group_src))
-    comm = _comm_for(group)
+    comm, peer = _resolve("irecv", group, False, "src", src, group_src, default=_ANY_SOURCE, translate_first=False)
     if comm is None:
         return _not_in_group("irecv")
-    if src is None and group_src is None:
-        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    if _is_group(group):
-        peer = _group_rank("irecv", "src", group, src, group_src)
-    else:
-        peer = _world_rank(src, group_src)
     return _p2p_batch([("recv", tensor, peer)], comm)
 
 
@@ -588,14 +588,10 @@ class P2POp:
             raise ValueError("Invalid ``op``. Expected ``op`` to be of type ``torch.distributed.isend`` or ``torch.distributed.irecv``.")
         self = super().__new__(cls)
         self.op, self.tensor, self.group, self.tag = op, tensor, group, tag
-        if _is_group(group):
-            if _is_non_member(group):  # torch translates the peer at construction, which a non-member cannot
-                raise ValueError("P2POp: this rank is not a member of the group, so its peer cannot be translated")
-            self.group_peer = _group_rank("P2POp", "peer", group, peer, group_peer, default=None)
-            self.peer = group.get_global_rank(self.group_peer)
-        else:
-            self.peer = _world_rank(peer, group_peer)
-            self.group_peer = self.peer
+        comm, self.group_peer = _resolve("P2POp", group, False, "peer", peer, group_peer, default=None, check=False)
+        if comm is None:  # torch translates the peer at construction, which a non-member cannot
+            raise ValueError("P2POp: this rank is not a member of the group, so its peer cannot be translated")
+        self.peer = _global_rank(group, self.group_peer)
         return self
 
 
@@ -612,33 +608,17 @@ def batch_isend_irecv(p2p_op_list: List[Any]) -> List[Any]:
     if len(p2p_op_list) > B2_P2P_MAX_OPS:
         raise ValueError(f"batch_isend_irecv: {len(p2p_op_list)} ops, the b200 communicator takes at most {B2_P2P_MAX_OPS} "
                          "in one batch")
-    group = p2p_op_list[0].group
-    ops = []
+    comm, ops = None, []
     for p in p2p_op_list:
-        if _is_group(group) or _is_group(p.group):
-            if p.group is not group:
-                raise ValueError("All ops need to use the same group.")
-            comm = _comm_for(group)
-            peer = p.group_peer
-        else:
-            _check_native_call(p.group, False)
-            comm = _COMM
-            peer = p.peer
-        if peer is None:
-            raise NotImplementedError("the b200 communicator cannot receive from any source: pass peer")
-        ops.append(("send" if p.op in (isend, dist.isend) else "recv", p.tensor, peer))
+        c, _ = _resolve("batch_isend_irecv", p.group)
+        if ops and c is not comm:
+            raise ValueError("All ops need to use the same group.")
+        if p.group_peer is None:
+            raise NotImplementedError(_NO_ANY_SOURCE)
+        comm = c
+        ops.append(("send" if p.op in (isend, dist.isend) else "recv", p.tensor, p.group_peer))
     work = _p2p_batch(ops, comm)
     return [work] * len(ops)
-
-
-def _check_rank(name: str, r: Any, world: Optional[int] = None) -> int:
-    from torchx_b200.ddp.comm import as_rank
-
-    world = _COMM.world if world is None else world
-    k = as_rank(r)
-    if k is None or not 0 <= k < world:
-        raise ValueError(f"{name} {r!r} is not a rank of a world of {world}")
-    return k
 
 
 def gather(tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]] = None, dst: Optional[int] = None, group: Any = None,
@@ -649,25 +629,27 @@ def gather(tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]] = Non
     if not _on_fabric():
         return dist.gather(tensor, gather_list, dst=0 if dst is None and group_dst is None else dst, group=group, async_op=async_op,
                            **_given(group_dst=group_dst))
-    comm = _comm_for(group, async_op)
+    comm, dst = _resolve("gather", group, async_op, "dst", dst, group_dst, translate_first=False)
     if comm is None:
         return _not_in_group("gather")
-    if _is_group(group):
-        dst = _group_rank("gather", "dst", group, dst, group_dst)
-    else:
-        dst = _check_rank("gather: dst", _world_rank(0 if dst is None and group_dst is None else dst, group_dst))
-    if comm.rank != dst:
-        if gather_list:
-            raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
-        comm.p2p_([("send", tensor, dst)])
-        return None
-    if not gather_list:
-        raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
-    _check_list("gather: gather_list", gather_list, tensor, comm.world)
-    if comm.world > 1:
-        comm.p2p_([("recv", t, r) for r, t in enumerate(gather_list) if r != dst])
-    gather_list[dst].copy_(tensor)
+    _gather(comm, tensor, gather_list, dst)(None)
     return None
+
+
+def _gather(comm: Any, tensor: torch.Tensor, gather_list: Optional[List[torch.Tensor]], dst: int) -> Callable[[Any], None]:
+    """``gather``'s checks on ``comm``, and its ``launch(stream)``: rank ``dst`` receives W - 1 messages in one batch and
+    copies its own tensor; every other rank sends one."""
+    _check_root_list(comm.rank == dst, gather_list, "gather_list", "destination")
+    if comm.rank != dst:
+        return lambda stream: comm.p2p_([("send", tensor, dst)], **_on(stream))
+    _check_list("gather: gather_list", gather_list, tensor, comm.world, "gather: gather_list: every tensor")
+
+    def launch(stream: Any) -> None:
+        if comm.world > 1:
+            comm.p2p_([("recv", t, r) for r, t in enumerate(gather_list) if r != dst], **_on(stream))
+        gather_list[dst].copy_(tensor)
+
+    return launch
 
 
 def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = None, src: Optional[int] = None, group: Any = None,
@@ -678,34 +660,44 @@ def scatter(tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]] = N
     if not _on_fabric():
         return dist.scatter(tensor, scatter_list, src=0 if src is None and group_src is None else src, group=group,
                             async_op=async_op, **_given(group_src=group_src))
-    comm = _comm_for(group, async_op)
-    if _is_group(group):
-        src = _group_rank("scatter", "src", group, src, group_src)
-        if comm is None:
-            return _not_in_group("scatter")
-    else:
-        src = _check_rank("scatter: src", _world_rank(0 if src is None and group_src is None else src, group_src))
-    if comm.rank != src:
-        if scatter_list:
-            raise ValueError("Argument ``scatter_list`` must NOT be specified on non-source ranks.")
-        comm.p2p_([("recv", tensor, src)])
-        return None
-    if not scatter_list:
-        raise ValueError("Argument ``scatter_list`` must be specified on source rank.")
-    _check_list("scatter: scatter_list", scatter_list, tensor, comm.world)
-    if comm.world > 1:
-        comm.p2p_([("send", t, r) for r, t in enumerate(scatter_list) if r != src])
-    tensor.copy_(scatter_list[src])
+    comm, src = _resolve("scatter", group, async_op, "src", src, group_src)
+    if comm is None:
+        return _not_in_group("scatter")
+    _scatter(comm, tensor, scatter_list, src)(None)
     return None
 
 
-def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor, world: Optional[int] = None) -> None:
-    world = _COMM.world if world is None else world
+def _scatter(comm: Any, tensor: torch.Tensor, scatter_list: Optional[List[torch.Tensor]], src: int) -> Callable[[Any], None]:
+    """``scatter``'s checks on ``comm``, and its ``launch(stream)``: rank ``src`` sends W - 1 messages in one batch and
+    copies its own block; every other rank receives one."""
+    _check_root_list(comm.rank == src, scatter_list, "scatter_list", "source")
+    if comm.rank != src:
+        return lambda stream: comm.p2p_([("recv", tensor, src)], **_on(stream))
+    _check_list("scatter: scatter_list", scatter_list, tensor, comm.world, "scatter: scatter_list: every tensor")
+
+    def launch(stream: Any) -> None:
+        if comm.world > 1:
+            comm.p2p_([("send", t, r) for r, t in enumerate(scatter_list) if r != src], **_on(stream))
+        tensor.copy_(scatter_list[src])
+
+    return launch
+
+
+def _check_root_list(root: bool, given: Any, name: str, role: str) -> None:
+    """The list argument ``name`` is given on the root (the ``role`` rank) and only there, as torch requires."""
+    if root and not given:
+        raise ValueError(f"Argument ``{name}`` must be specified on {role} rank.")
+    if not root and given:
+        raise ValueError(f"Argument ``{name}`` must NOT be specified on non-{role} ranks.")
+
+
+def _check_list(what: str, tensors: List[torch.Tensor], like: torch.Tensor, world: int, every: str) -> None:
+    """``tensors`` are world tensors of ``like``'s dtype and size; ``what`` and ``every`` name them in the errors."""
     if len(tensors) != world:
         raise ValueError(f"{what} has {len(tensors)} tensors, world size is {world}")
     for t in tensors:
         if t.dtype != like.dtype or t.numel() != like.numel():
-            raise ValueError(f"{what}: every tensor must be {like.dtype} with {like.numel()} elements")
+            raise ValueError(f"{every} must be {like.dtype} with {like.numel()} elements")
 
 
 def reduce(tensor: torch.Tensor, dst: Optional[int] = None, op: Any = dist.ReduceOp.SUM, group: Any = None,
@@ -715,13 +707,9 @@ def reduce(tensor: torch.Tensor, dst: Optional[int] = None, op: Any = dist.Reduc
     same op leaves (include/b200ddp.h: b2_reduce), and each rank sends (W-1)/W of the tensor."""
     if not _on_fabric():
         return dist.reduce(tensor, dst, op=op, group=group, async_op=async_op, **_given(group_dst=group_dst))
-    comm = _comm_for(group, async_op)
-    if _is_group(group):
-        dst = _group_rank("reduce", "dst", group, dst, group_dst, default=None)
-        if comm is None:
-            return _not_in_group("reduce")
-    else:
-        dst = _check_rank("reduce: dst", _world_rank(dst, group_dst))
+    comm, dst = _resolve("reduce", group, async_op, "dst", dst, group_dst, default=None)
+    if comm is None:
+        return _not_in_group("reduce")
     comm.reduce_(tensor, dst, reduce_op_name(op))
     return None
 
@@ -737,11 +725,9 @@ def _comm_device() -> torch.device:
     return torch.device("cuda", _COMM.device)
 
 
-def _check_object_call(fn: str, group: Any, device: Any = None) -> torch.device:
-    """The device an object collective runs on: the communicator's.  ``group`` must be None, WORLD or a ``B200Group`` (or
-    ``NON_GROUP_MEMBER``) and ``device``, if given, the communicator's device: the fabric never moves the exchange
-    elsewhere."""
-    _comm_for(group)
+def _object_device(fn: str, device: Any = None) -> torch.device:
+    """The device an object collective runs on: the communicator's.  ``device``, if given, must be that device: the fabric
+    never moves the exchange elsewhere."""
     here = _comm_device()
     if device is not None:
         d = torch.device(device)
@@ -750,22 +736,6 @@ def _check_object_call(fn: str, group: Any, device: Any = None) -> torch.device:
         if d != here:
             raise ValueError(f"{fn}: device {device} is not the b200 communicator's device {here}")
     return here
-
-
-def _peer_arg(fn: str, name: str, r: Any, group_r: Any, default: Optional[int] = 0, group: Any = None) -> int:
-    """``src`` / ``dst`` of an object collective, as a rank of ``group``'s communicator.  On the world ``group_src`` /
-    ``group_dst`` may stand in for it or repeat it (the world's group rank is the rank); on a group see ``_group_rank``."""
-    if _is_group(group):
-        return _group_rank(fn, name, group, r, group_r, default)
-    if group_r is not None:
-        if r is not None and r != group_r:
-            raise ValueError(f"{fn}: group_{name} {group_r!r} differs from {name} {r!r}; the b200 communicator has no subgroups")
-        r = group_r
-    if r is None:
-        if default is None:
-            raise ValueError(f"{fn}: {name} must be given")
-        r = default
-    return _check_rank(f"{fn}: {name}", r)
 
 
 def _to_bytes(obj: Any, device: torch.device) -> torch.Tensor:
@@ -784,12 +754,29 @@ def _concat_sizes(tensors: List[torch.Tensor], device: torch.device):
     return sizes, (torch.cat(tensors) if len(tensors) != 1 else tensors[0])
 
 
-def _split_objects(object_list: List[Any], sizes: List[int], data: torch.Tensor) -> None:
+def _load_objects(object_list: List[Any], data: torch.Tensor, sizes: List[int], block: Optional[int] = None) -> None:
+    """``object_list[i]`` <- the object pickled in the i-th ``sizes[i]`` bytes of ``data``: packed one after another, or
+    each at the start of a padded block of ``block`` bytes."""
     host = data.cpu().numpy().tobytes()
     at = 0
     for i, n in enumerate(sizes):
         object_list[i] = pickle.loads(host[at: at + n])
-        at += n
+        at += n if block is None else block
+
+
+def _exchange_padded(comm: Any, obj: Any, device: torch.device, object_list: Optional[List[Any]],
+                     exchange: Callable[[torch.Tensor, int], Optional[torch.Tensor]]) -> None:
+    """All-gather every rank's pickled size, then ``exchange(this rank's bytes padded to the largest size, that size)``,
+    which returns the W padded blocks in rank order (or None on a rank that receives nothing), unpickled into
+    ``object_list``."""
+    mine = _to_bytes(obj, device)
+    sizes = torch.empty(comm.world, dtype=torch.int64, device=device)
+    comm.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
+    sizes = sizes.tolist()
+    block = max(sizes)
+    out = exchange(_padded(mine, block), block)
+    if out is not None:
+        _load_objects(object_list, out, sizes, block)
 
 
 def all_gather_object(object_list: List[Any], obj: Any, group: Any = None) -> None:
@@ -797,21 +784,17 @@ def all_gather_object(object_list: List[Any], obj: Any, group: Any = None) -> No
     ``init_pg("b200")``: one all-gather of the sizes, one of the padded bytes.  Unpickling trusts every peer."""
     if not _on_fabric():
         return dist.all_gather_object(object_list, obj, group=group)
-    device = _check_object_call("all_gather_object", group)
-    comm = _comm_for(group)
+    comm, _ = _resolve("all_gather_object", group)
+    device = _object_device("all_gather_object")
     if comm is None:
         return _not_in_group("all_gather_object")
-    W = comm.world
-    mine = _to_bytes(obj, device)
-    sizes = torch.empty(W, dtype=torch.int64, device=device)
-    comm.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
-    sizes = sizes.tolist()
-    block = max(sizes)
-    out = torch.empty(W * block, dtype=torch.uint8, device=device)
-    comm.allgather_(out, _padded(mine, block))
-    host = out.cpu().numpy().tobytes()
-    for r in range(W):
-        object_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
+
+    def exchange(padded: torch.Tensor, block: int) -> torch.Tensor:
+        out = torch.empty(comm.world * block, dtype=torch.uint8, device=device)
+        comm.allgather_(out, padded)
+        return out
+
+    _exchange_padded(comm, obj, device, object_list, exchange)
     return None
 
 
@@ -822,30 +805,18 @@ def gather_object(obj: Any, object_gather_list: Optional[List[Any]] = None, dst:
     Unpickling trusts every peer."""
     if not _on_fabric():
         return dist.gather_object(obj, object_gather_list, dst=dst, group=group, group_dst=group_dst)
-    device = _check_object_call("gather_object", group)
-    comm = _comm_for(group)
-    dst = _peer_arg("gather_object", "dst", dst, group_dst, group=group)
+    comm, dst = _resolve("gather_object", group, False, "dst", dst, group_dst)
+    device = _object_device("gather_object")
     if comm is None:
         return _not_in_group("gather_object")
-    if comm.rank == dst and not object_gather_list:
-        raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
-    if comm.rank != dst and object_gather_list:
-        raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
-    W = comm.world
-    mine = _to_bytes(obj, device)
-    sizes = torch.empty(W, dtype=torch.int64, device=device)
-    comm.allgather_(sizes, torch.tensor([mine.numel()], dtype=torch.int64).to(device))
-    sizes = sizes.tolist()
-    block = max(sizes)
-    grp = group if _is_group(group) else None
-    if comm.rank != dst:
-        gather(_padded(mine, block), None, group=grp, group_dst=dst)
-        return None
-    out = torch.empty(W, block, dtype=torch.uint8, device=device)
-    gather(_padded(mine, block), list(out.unbind(0)), group=grp, group_dst=dst)
-    host = out.cpu().numpy().tobytes()
-    for r in range(W):
-        object_gather_list[r] = pickle.loads(host[r * block: r * block + sizes[r]])
+    _check_root_list(comm.rank == dst, object_gather_list, "gather_list", "destination")
+
+    def exchange(padded: torch.Tensor, block: int) -> Optional[torch.Tensor]:
+        out = torch.empty(comm.world, block, dtype=torch.uint8, device=device) if comm.rank == dst else None
+        _gather(comm, padded, None if out is None else list(out.unbind(0)), dst)(None)
+        return out
+
+    _exchange_padded(comm, obj, device, object_gather_list, exchange)
     return None
 
 
@@ -856,9 +827,8 @@ def broadcast_object_list(object_list: List[Any], src: Optional[int] = None, gro
     sizes, one of the concatenated bytes.  Unpickling trusts rank ``src``."""
     if not _on_fabric():
         return dist.broadcast_object_list(object_list, src=src, group=group, device=device, group_src=group_src)
-    dev = _check_object_call("broadcast_object_list", group, device)
-    comm = _comm_for(group)
-    src = _peer_arg("broadcast_object_list", "src", src, group_src, group=group)
+    comm, src = _resolve("broadcast_object_list", group, False, "src", src, group_src)
+    dev = _object_device("broadcast_object_list", device)
     if comm is None:
         return _not_in_group("broadcast_object_list")
     if comm.rank == src:
@@ -871,7 +841,7 @@ def broadcast_object_list(object_list: List[Any], src: Optional[int] = None, gro
     sizes = sizes.tolist()
     data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
     comm.broadcast_(data, root=src)
-    _split_objects(object_list, sizes, data)
+    _load_objects(object_list, data, sizes)
     return None
 
 
@@ -883,15 +853,13 @@ def scatter_object_list(scatter_object_output_list: List[Any], scatter_object_in
     if not _on_fabric():
         return dist.scatter_object_list(scatter_object_output_list, scatter_object_input_list, src=src, group=group,
                                         group_src=group_src)
-    device = _check_object_call("scatter_object_list", group)
-    comm = _comm_for(group)
-    src = _peer_arg("scatter_object_list", "src", src, group_src, group=group)
+    comm, src = _resolve("scatter_object_list", group, False, "src", src, group_src)
+    device = _object_device("scatter_object_list")
     if comm is None:
         return _not_in_group("scatter_object_list")
     if not isinstance(scatter_object_output_list, list) or len(scatter_object_output_list) < 1:
         raise ValueError("Expected argument scatter_object_output_list to be a list of size at least 1.")
     W = comm.world
-    grp = group if _is_group(group) else None
     if comm.rank == src:
         if scatter_object_input_list is None:
             raise ValueError("source rank must provide non-None scatter_object_input_list")
@@ -902,16 +870,16 @@ def scatter_object_list(scatter_object_output_list: List[Any], scatter_object_in
         comm.broadcast_(torch.tensor([t.numel() for t in parts], dtype=torch.int64).to(device), root=src)
         block = max(t.numel() for t in parts)
         out = torch.empty(block, dtype=torch.uint8, device=device)
-        scatter(out, [_padded(t, block) for t in parts], group=grp, group_src=src)
+        _scatter(comm, out, [_padded(t, block) for t in parts], src)(None)
         n = parts[src].numel()
     else:
         sizes = torch.empty(W, dtype=torch.int64, device=device)
         comm.broadcast_(sizes, root=src)
         sizes = sizes.tolist()
         out = torch.empty(max(sizes), dtype=torch.uint8, device=device)
-        scatter(out, None, group=grp, group_src=src)
+        _scatter(comm, out, None, src)(None)
         n = sizes[comm.rank]
-    scatter_object_output_list[0] = pickle.loads(out[:n].cpu().numpy().tobytes())
+    _load_objects(scatter_object_output_list, out, [n])
     return None
 
 
@@ -921,9 +889,10 @@ def send_object_list(object_list: List[Any], dst: Optional[int] = None, group: A
     ``init_pg("b200")``: one send of the sizes, one of the concatenated bytes; ``use_batch`` is accepted and ignored."""
     if not _on_fabric():
         return dist.send_object_list(object_list, dst=dst, group=group, device=device, group_dst=group_dst, use_batch=use_batch)
-    dev = _check_object_call("send_object_list", group, device)
-    comm = _comm_for(group)
-    dst = _peer_arg("send_object_list", "dst", dst, group_dst, default=None, group=group)
+    if dst is None and group_dst is None:
+        raise ValueError("send_object_list: dst must be given")
+    comm, dst = _resolve("send_object_list", group, False, "dst", dst, group_dst)
+    dev = _object_device("send_object_list", device)
     if comm is None:
         return _not_in_group("send_object_list")
     sizes, data = _concat_sizes([_to_bytes(o, dev) for o in object_list], dev)
@@ -939,11 +908,8 @@ def recv_object_list(object_list: List[Any], src: Optional[int] = None, group: A
     fabric.  Unpickling trusts rank ``src``."""
     if not _on_fabric():
         return dist.recv_object_list(object_list, src=src, group=group, device=device, group_src=group_src, use_batch=use_batch)
-    dev = _check_object_call("recv_object_list", group, device)
-    comm = _comm_for(group)
-    if src is None and group_src is None:
-        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
-    src = _peer_arg("recv_object_list", "src", src, group_src, group=group)
+    comm, src = _resolve("recv_object_list", group, False, "src", src, group_src, default=_ANY_SOURCE)
+    dev = _object_device("recv_object_list", device)
     if comm is None:
         return _not_in_group("recv_object_list", -1)
     sizes = torch.empty(len(object_list), dtype=torch.int64, device=dev)
@@ -951,8 +917,8 @@ def recv_object_list(object_list: List[Any], src: Optional[int] = None, group: A
     sizes = sizes.tolist()
     data = torch.empty(sum(sizes), dtype=torch.uint8, device=dev)
     comm.p2p_([("recv", data, src)])
-    _split_objects(object_list, sizes, data)
-    return group.get_global_rank(src) if isinstance(group, B200Group) else src
+    _load_objects(object_list, data, sizes)
+    return _global_rank(group, src)
 
 
 @contextmanager

@@ -26,13 +26,11 @@ import torch
 import torch.distributed as dist
 from torch._C._distributed_c10d import _create_work_from_future
 
+from torchx_b200 import distributed as D
+from torchx_b200.ddp._native import B2_P2P_MAX_OPS
+from torchx_b200.ddp.comm import check_allgather, check_alltoall, check_peer, check_reduce_scatter, dtype_op_for
+
 BACKEND = "b200"
-
-
-def _d():
-    from torchx_b200 import distributed as D
-
-    return D
 
 
 class B200ProcessGroup(dist.ProcessGroup):
@@ -86,11 +84,12 @@ class B200ProcessGroup(dist.ProcessGroup):
         return _create_work_from_future(fut)
 
     def _op(self, op: Any, dtype: torch.dtype, fn: str) -> str:
-        from torchx_b200.ddp.comm import dtype_op_for
-
-        name = _d().reduce_op_name(op)
+        name = D.reduce_op_name(op)
         dtype_op_for(dtype, name, fn)
         return name
+
+    def _root(self, fn: str, name: str, opts: Any) -> int:
+        return D._resolve(fn, None, name=name, r=opts.rootRank, world=self.comm)[1]
 
     @staticmethod
     def _one(tensors: Sequence[torch.Tensor], fn: str) -> torch.Tensor:
@@ -109,95 +108,55 @@ class B200ProcessGroup(dist.ProcessGroup):
     def broadcast(self, tensors: List[torch.Tensor], opts: Any) -> Any:
         self._guard()
         t = self._one(tensors, "broadcast")
-        root = _d()._check_rank("broadcast: src", opts.rootRank)
+        root = self._root("broadcast", "src", opts)
         self._check([t])
         return self._enqueue(lambda s: self.comm.broadcast_(t, root=root, stream=s), [t], [t])
 
     def _allgather_base(self, output: torch.Tensor, input: torch.Tensor, opts: Any = None) -> Any:  # noqa: A002
         self._guard()
-        if output.dtype != input.dtype:
-            raise TypeError(f"allgather_: out is {output.dtype}, input is {input.dtype}")
-        self._check([output, input])
-        if output.numel() != self.comm.world * input.numel():
-            raise ValueError(f"allgather_: out has {output.numel()} elements, needs {self.comm.world} x {input.numel()}")
+        check_allgather(self.comm, output, input)
         return self._enqueue(lambda s: self.comm.allgather_(output, input, stream=s), [output, input], [output])
 
     def allgather(self, output_tensors: List[List[torch.Tensor]], input_tensors: List[torch.Tensor], opts: Any = None) -> Any:
         self._guard()
         t = self._one(input_tensors, "allgather")
         outs = self._one(output_tensors, "allgather")
-        W = self.comm.world
-        if len(outs) != W:
-            raise ValueError(f"all_gather: tensor_list has {len(outs)} tensors, world size is {W}")
-        for o in outs:
-            if o.dtype != t.dtype or o.numel() != t.numel():
-                raise ValueError(f"all_gather: every tensor of tensor_list must be {t.dtype} with {t.numel()} elements")
+        launch = D._all_gather(self.comm, outs, t)
         self._check([t, *outs])
-
-        def launch(s):  # one all-gather into a staging buffer, then a copy per rank, as D.all_gather does
-            flat = torch.empty((W,) + tuple(t.shape), dtype=t.dtype, device=t.device)
-            self.comm.allgather_(flat, t, stream=s)
-            for r, o in enumerate(outs):
-                o.copy_(flat[r].view_as(o))
-
         return self._enqueue(launch, [t, *outs], list(outs))
 
     def _reduce_scatter_base(self, output: torch.Tensor, input: torch.Tensor, opts: Any) -> Any:  # noqa: A002
         self._guard()
-        name = self._op(opts.reduceOp, input.dtype, "reduce_scatter_")
-        if output.dtype != input.dtype:
-            raise TypeError(f"reduce_scatter_: out is {output.dtype}, input is {input.dtype}")
-        if input.numel() != self.comm.world * output.numel():
-            raise ValueError(f"reduce_scatter_: input has {input.numel()} elements, needs {self.comm.world} x {output.numel()}")
-        self._check([output, input])
+        name = D.reduce_op_name(opts.reduceOp)
+        check_reduce_scatter(self.comm, output, input, name)
         return self._enqueue(lambda s: self.comm.reduce_scatter_(output, input, name, stream=s), [output, input], [output])
 
     def reduce_scatter(self, output_tensors: List[torch.Tensor], input_tensors: List[List[torch.Tensor]], opts: Any) -> Any:
         self._guard()
         out = self._one(output_tensors, "reduce_scatter")
         ins = self._one(input_tensors, "reduce_scatter")
-        name = self._op(opts.reduceOp, out.dtype, "reduce_scatter_")
-        W = self.comm.world
-        if len(ins) != W:
-            raise ValueError(f"reduce_scatter: input_list has {len(ins)} tensors, world size is {W}")
-        for t in ins:
-            if t.dtype != out.dtype or t.numel() != out.numel():
-                raise ValueError(f"reduce_scatter: every tensor of input_list must be {out.dtype} with {out.numel()} elements")
+        launch = D._reduce_scatter(self.comm, out, ins, self._op(opts.reduceOp, out.dtype, "reduce_scatter_"))
         self._check([out, *ins])
-
-        def launch(s):
-            self.comm.reduce_scatter_(out, torch.cat([t.reshape(-1) for t in ins]), name, stream=s)
-
         return self._enqueue(launch, [out, *ins], [out])
 
     def reduce(self, tensors: List[torch.Tensor], opts: Any) -> Any:
         self._guard()
         t = self._one(tensors, "reduce")
         name = self._op(opts.reduceOp, t.dtype, "reduce_")
-        root = _d()._check_rank("reduce: dst", opts.rootRank)
+        root = self._root("reduce", "dst", opts)
         self._check([t])
         return self._enqueue(lambda s: self.comm.reduce_(t, root, name, stream=s), [t], [t])
 
     def alltoall_base(self, output: torch.Tensor, input: torch.Tensor, output_split_sizes: List[int],  # noqa: A002
                       input_split_sizes: List[int], opts: Any = None) -> Any:
         self._guard()
-        D = _d()
         self._check([output, input])
-        outs = D._split_rows(output, output_split_sizes, "output", self.comm.world)
-        ins = D._split_rows(input, input_split_sizes, "input", self.comm.world)
-        if output.dtype != input.dtype:
-            raise TypeError(f"alltoall_: every tensor must have one dtype, got {sorted({str(output.dtype), str(input.dtype)})}")
-        return self._enqueue(lambda s: self.comm.alltoall_(outs, ins, stream=s), [output, input], [output])
+        launch = D._all_to_all_single(self.comm, output, input, output_split_sizes, input_split_sizes)
+        return self._enqueue(launch, [output, input], [output])
 
     def alltoall(self, output_tensors: List[torch.Tensor], input_tensors: List[torch.Tensor], opts: Any = None) -> Any:
         self._guard()
-        W = self.comm.world
-        if len(output_tensors) != W or len(input_tensors) != W:
-            raise ValueError(f"alltoall_: needs {W} output and {W} input tensors, got {len(output_tensors)} and "
-                             f"{len(input_tensors)}")
-        dtypes = {t.dtype for t in (*output_tensors, *input_tensors)}
-        if len(dtypes) > 1:
-            raise TypeError(f"alltoall_: every tensor must have one dtype, got {sorted(str(d) for d in dtypes)}")
+        check_alltoall(self.comm.world, output_tensors, input_tensors)
         self._check([*output_tensors, *input_tensors])
         outs, ins = list(output_tensors), list(input_tensors)
         return self._enqueue(lambda s: self.comm.alltoall_(outs, ins, stream=s), [*outs, *ins], outs)
@@ -208,13 +167,8 @@ class B200ProcessGroup(dist.ProcessGroup):
         so the batch reads and writes the tensor after the work issued before this call."""
         self._guard(flush=False)
         t = self._one(tensors, kind)
-        p = _d()._check_rank(f"{kind}: peer", peer)
-        if p == self.comm.rank:
-            raise ValueError(f"p2p_: op 0 names peer {peer!r}; rank {self.comm.rank} of {self.comm.world} can only name "
-                             "another rank")
+        p = check_peer(0, peer, self.comm.rank, self.comm.world)
         self._check([t])
-        from torchx_b200.ddp._native import B2_P2P_MAX_OPS
-
         if len(self._pending) == B2_P2P_MAX_OPS:
             self._flush()
         self._wait_current()
@@ -240,54 +194,26 @@ class B200ProcessGroup(dist.ProcessGroup):
         return self._p2p("recv", tensors, srcRank)
 
     def recv_anysource(self, tensors: List[torch.Tensor], tag: int = 0) -> Any:
-        raise NotImplementedError("the b200 communicator cannot receive from any source: pass src")
+        raise NotImplementedError(D._NO_ANY_SOURCE)
 
     def gather(self, output_tensors: List[List[torch.Tensor]], input_tensors: List[torch.Tensor], opts: Any) -> Any:
         """``D.gather``'s batches: the root receives W - 1 messages in one launch and copies its own tensor."""
         self._guard()
         t = self._one(input_tensors, "gather")
-        dst = _d()._check_rank("gather: dst", opts.rootRank)
-        comm = self.comm
-        if comm.rank != dst:
-            if output_tensors and any(output_tensors):
-                raise ValueError("Argument ``gather_list`` must NOT be specified on non-destination ranks.")
-            self._check([t])
-            return self._enqueue(lambda s: comm.p2p_([("send", t, dst)], stream=s), [t], [])
-        gl = self._one(output_tensors, "gather") if output_tensors else []
-        if not gl:
-            raise ValueError("Argument ``gather_list`` must be specified on destination rank.")
-        _d()._check_list("gather: gather_list", gl, t, comm.world)
+        dst = self._root("gather", "dst", opts)
+        gl = self._one(output_tensors, "gather") if output_tensors and any(output_tensors) else []
+        launch = D._gather(self.comm, t, gl, dst)
         self._check([t, *gl])
-
-        def launch(s):
-            if comm.world > 1:
-                comm.p2p_([("recv", o, r) for r, o in enumerate(gl) if r != dst], stream=s)
-            gl[dst].copy_(t)
-
         return self._enqueue(launch, [t, *gl], list(gl))
 
     def scatter(self, output_tensors: List[torch.Tensor], input_tensors: List[List[torch.Tensor]], opts: Any) -> Any:
         """``D.scatter``'s batches: the root sends W - 1 messages in one launch and copies its own block."""
         self._guard()
         t = self._one(output_tensors, "scatter")
-        src = _d()._check_rank("scatter: src", opts.rootRank)
-        comm = self.comm
-        if comm.rank != src:
-            if input_tensors and any(input_tensors):
-                raise ValueError("Argument ``scatter_list`` must NOT be specified on non-source ranks.")
-            self._check([t])
-            return self._enqueue(lambda s: comm.p2p_([("recv", t, src)], stream=s), [t], [t])
-        sl = self._one(input_tensors, "scatter") if input_tensors else []
-        if not sl:
-            raise ValueError("Argument ``scatter_list`` must be specified on source rank.")
-        _d()._check_list("scatter: scatter_list", sl, t, comm.world)
+        src = self._root("scatter", "src", opts)
+        sl = self._one(input_tensors, "scatter") if input_tensors and any(input_tensors) else []
+        launch = D._scatter(self.comm, t, sl, src)
         self._check([t, *sl])
-
-        def launch(s):
-            if comm.world > 1:
-                comm.p2p_([("send", x, r) for r, x in enumerate(sl) if r != src], stream=s)
-            t.copy_(sl[src])
-
         return self._enqueue(launch, [t, *sl], [t])
 
     def barrier(self, opts: Any = None) -> Any:
@@ -348,13 +274,8 @@ class _P2PWork(dist.Work):
 def _create(opts: Any, pg_options: Any = None) -> B200ProcessGroup:
     """The creator ``init_process_group`` / ``new_group`` call: one group on the process communicator (``_COMM``, made from
     the environment if ``init_pg("b200")`` did not make it).  The store is not used."""
-    D = _d()
     ranks = list(opts.global_ranks_in_group)
-    if D._COMM is None:
-        from torchx_b200.ddp import Communicator
-
-        D._COMM = Communicator.from_env()
-    comm = D._COMM
+    comm = D.process_communicator()
     if ranks and sorted(ranks) != list(range(comm.world)):
         raise NotImplementedError("the b200 communicator has no subgroups: a b200 group must hold every rank")
     if opts.group_rank != comm.rank or opts.group_size != comm.world:

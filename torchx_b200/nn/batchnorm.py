@@ -13,7 +13,6 @@ from __future__ import annotations
 from typing import Any, Callable
 
 import torch
-import torch.distributed as dist
 import torch.nn.functional as F
 from torch import nn
 
@@ -121,14 +120,12 @@ class SyncBatchNorm(nn.SyncBatchNorm):
         bn_training = True if self.training else (self.running_mean is None) and (self.running_var is None)
         running_mean = self.running_mean if not self.training or self.track_running_stats else None
         running_var = self.running_var if not self.training or self.track_running_stats else None
-        comm = _dist.communicator()
         need_sync = bn_training and self.training
         if need_sync:
-            if isinstance(self.process_group, _dist.B200Group):
-                comm = self.process_group.comm  # the statistics of the group's ranks only, merged in group-rank order
-            elif self.process_group is not None and self.process_group is not dist.group.WORLD:
-                raise NotImplementedError("the b200 communicator has no subgroups but a B200Group: SyncBatchNorm needs "
-                                          "process_group=None or a torchx_b200.distributed.new_group group")
+            # a B200Group's communicator: the statistics of the group's ranks only, merged in group-rank order
+            comm, _ = _dist._resolve("SyncBatchNorm", self.process_group)
+            if comm is None:  # NON_GROUP_MEMBER
+                raise NotImplementedError(_dist._NO_SUBGROUPS)
             for name, t in (("running_mean", running_mean), ("running_var", running_var)):
                 if t is not None and t.dtype != torch.float32:
                     raise TypeError(f"SyncBatchNorm on the b200 communicator keeps float32 running statistics, {name} is {t.dtype}")
