@@ -54,8 +54,9 @@ extern "C" {
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
                             b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats,
-                            b2_bn_backward_reduce, b2_reduce, b2_reduce_scatter_step_bf16 and b2_comm_create_group, which only add symbols: a binding that needs them
-                            fails to resolve them against an older library */
+                            b2_bn_backward_reduce, b2_reduce, b2_reduce_scatter_step_bf16, b2_comm_create_group, b2_bn_forward_relu and
+                            b2_bn_backward_reduce_relu, which only add symbols: a binding that needs them fails to resolve them against an
+                            older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
 /* ---- return codes ---------------------------------------------------------------- */
@@ -518,6 +519,23 @@ int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* m
 int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t channels, int dtype, const float* mean, const float* invstd,
                           float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias, void* workspace, size_t workspace_bytes,
                           int device, void* stream);
+
+/*
+ * A ResNet block's BatchNorm with the ReLU (and residual add) that follow it, on the same [rows, channels] view, with the
+ * bits of the unfused composition: ATen's BatchNorm, then its bf16 add_ and relu_ (DESIGN.md 2.4).  The checks are those
+ * of the calls above; a given residual must be 16-byte aligned.
+ */
+/* save_invstd and the BatchNorm output as b2_bn_forward_elemt; y <- relu(bn + residual) (residual may be null): the BatchNorm
+ * output rounded to dtype, plus residual in float rounded to dtype, then max(., 0) with NaN kept. */
+int b2_bn_forward_relu(const void* x, const void* residual, void* y, size_t rows, size_t channels, int dtype, const float* weight,
+                       const float* bias, const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream);
+
+/* dy <- (z <= 0 ? +0 : dz), the gradient of the BatchNorm output given the gradient dz of its ReLU's output z (torch's
+ * threshold_backward; also the residual's gradient), then b2_bn_backward_reduce's sums over dy, with the same bits.  dy may be
+ * dz (in place). */
+int b2_bn_backward_reduce_relu(const void* dz, const void* z, const void* x, void* dy, size_t rows, size_t channels, int dtype,
+                               const float* mean, const float* invstd, float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias,
+                               void* workspace, size_t workspace_bytes, int device, void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

@@ -12,7 +12,8 @@ under ``torch.profiler`` with CUDA activities, after a warm-up, and reports:
 * for every BatchNorm input shape [M = N*H*W, C]: the bytes an unfused BatchNorm must move (forward statistics read x,
   forward normalise read x + write y, backward reduce read x + dy, backward elementwise read x + dy + write dx: 8 passes
   of 2 B per element) over the measured time of those kernels, in GB/s and as a fraction of the H100 SXM data sheet's
-  3.35 TB/s.
+  3.35 TB/s.  A layer whose ReLU runs inside its passes (``torchx_b200.nn.resnet``) moves more: its backward reduce also
+  reads z and writes dy (+4 B per element), and its normalise reads the residual where it adds one (+2 B per element).
 
 Kernels are matched to layers by their order within a step: forward kernels in module order, backward kernels in reverse.
 ``--tree DIR`` imports ``bench`` and ``torchx_b200`` from another checkout (a build of an earlier commit), so two versions
@@ -45,6 +46,9 @@ BN_PASSES = [
     ("bwd_reduce", re.compile(r"batch_norm_backward_reduce|k_bn2d_bwd_reduce\b"), 2, "bwd"),
     ("bwd_elemt", re.compile(r"batch_norm_backward_elemt|k_bn2d_bwd_elemt\b"), 3, "bwd"),
 ]
+# (pass, extra bytes per element of x) of a layer with the ReLU inside its passes, and of one that also adds the residual
+FUSED_EXTRA = {"bwd_reduce": 4}
+RESIDUAL_EXTRA = {"fwd_norm": 2}
 # The small second launch of a native reduction whose tree spans several CTA rows (it folds their partials): its time
 # belongs to the layer of the pass launched just before it
 BN_TAILS = [
@@ -93,10 +97,19 @@ def main() -> None:
     x = xh.to(tr.device).contiguous(memory_format=torch.channels_last)
     y = yh.to(tr.device)
 
-    # BatchNorm input shapes in forward order, from one hooked eval-mode forward (which leaves the running statistics alone)
-    shapes = []
-    hooks = [m.register_forward_hook(lambda m, i, o: shapes.append((i[0].shape[0] * i[0].shape[2] * i[0].shape[3], i[0].shape[1])))
-             for m in tr.ddp.module.modules() if isinstance(m, torch.nn.BatchNorm2d)]
+    # BatchNorm input shapes in forward order, from one hooked eval-mode forward (which leaves the running statistics alone),
+    # and which layers a fused ResNet block (the class attributes of torchx_b200.nn.resnet's blocks) runs with their ReLU
+    fused = {}
+    for m in tr.ddp.module.modules():
+        for name in getattr(type(m), "_fused_bns", ()):
+            fused[id(getattr(m, name))] = "residual" if name == type(m)._residual_bn else "relu"
+    shapes, kinds = [], []
+
+    def record(m, i, o):
+        shapes.append((i[0].shape[0] * i[0].shape[2] * i[0].shape[3], i[0].shape[1]))
+        kinds.append(fused.get(id(m)))
+
+    hooks = [m.register_forward_hook(record) for m in tr.ddp.module.modules() if isinstance(m, torch.nn.BatchNorm2d)]
     tr.ddp.module.eval()
     with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
         tr.ddp.module(x)
@@ -152,13 +165,15 @@ def main() -> None:
     total_us = sum(per_group.values()) / S
     rows = []
     for (M, C) in sorted(set(shapes), key=lambda s: -s[0] * s[1]):
-        nl = shapes.count((M, C))
+        layers = [kinds[k] for k in range(L) if shapes[k] == (M, C)]
+        nl = len(layers)
         t = per_shape[(M, C)]
-        row = {"M": M, "C": C, "layers": nl, "MiB_bf16": round(M * C * 2 / 2**20, 1)}
+        row = {"M": M, "C": C, "layers": nl, "fused_layers": sum(1 for k in layers if k), "MiB_bf16": round(M * C * 2 / 2**20, 1)}
         tot_b, tot_t = 0, 0.0
         for pname, _, bpe, _ in BN_PASSES:
             us = t[pname] / S
-            b = bpe * 2 * M * C * nl
+            b = sum(bpe * 2 + (FUSED_EXTRA.get(pname, 0) if k else 0) + (RESIDUAL_EXTRA.get(pname, 0) if k == "residual" else 0)
+                    for k in layers) * M * C
             row[pname + "_us"] = round(us, 1)
             row[pname + "_gbs"] = round(b / (us * 1e-6) / 1e9, 1) if us > 0 else None
             tot_b += b
@@ -181,10 +196,10 @@ def main() -> None:
     for g, v in per_group.most_common():
         lines.append(f"| {g} | {v / S / 1e3:.2f} | {v / S / 1e3 / step_ms:.1%} |")
     lines += ["", f"BatchNorm layers: {L}; every pass matched S x L kernels: {bn_launch_ok}.", "",
-              "| M | C | layers | MiB bf16 | fwd stats GB/s | fwd norm GB/s | bwd reduce GB/s | bwd elemt GB/s | all 8 passes GB/s | of 3.35 TB/s |",
-              "|---:|---:|---:|---:|---:|---:|---:|---:|---:|---:|"]
+              "| M | C | layers | fused | MiB bf16 | fwd stats GB/s | fwd norm GB/s | bwd reduce GB/s | bwd elemt GB/s | all passes GB/s | of 3.35 TB/s |",
+              "|---:|---:|---:|---:|---:|---:|---:|---:|---:|---:|---:|"]
     for r in rows:
-        lines.append(f"| {r['M']} | {r['C']} | {r['layers']} | {r['MiB_bf16']} | {r['fwd_stats_gbs']} | {r['fwd_norm_gbs']} | "
+        lines.append(f"| {r['M']} | {r['C']} | {r['layers']} | {r['fused_layers']} | {r['MiB_bf16']} | {r['fwd_stats_gbs']} | {r['fwd_norm_gbs']} | "
                      f"{r['bwd_reduce_gbs']} | {r['bwd_elemt_gbs']} | {r['all_gbs']} | {r['all_frac']} |")
     lines += ["", "| kernel | ms / step |", "|---|---:|"] + [f"| `{n}` | {v} |" for n, v in res["top_kernels_ms_per_step"]]
     text = "\n".join(lines) + "\n"

@@ -1944,27 +1944,74 @@ int bn_check_workspace(const char* fn, const void* ws, size_t have, size_t need)
   return B2_OK;
 }
 
+// b2_bn_forward_elemt (residual null, no relu) and b2_bn_forward_relu.
+int bn_forward(const char* fn, const void* x, const void* residual, void* y, bool relu, size_t rows, size_t channels, int dtype,
+               const float* weight, const float* bias, const float* mean, const float* var, double eps, float* save_invstd, int device,
+               void* stream) {
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"y", y, 16}, {"weight", weight, 4}, {"bias", bias, 4}, {"mean", mean, 4},
+                                        {"var", var, 4}, {"save_invstd", save_invstd, 4}}))
+    return rc;
+  if (residual)
+    if (const int rc = bn_check_ptrs(fn, {{"residual", residual, 16}})) return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // k_bn2d_norm walks x and a residual kBnFwdUnroll / 2 rows at a time
+  const bn::Plan p = bn::plan(rows, channels, sm_count(device), residual ? kBnFwdUnroll / 2 : kBnFwdUnroll);
+  // ATen converts eps to float at its launch (acc_t); so does this call
+  k_bn2d_norm<kBnFwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(
+      static_cast<const uint16_t*>(x), static_cast<const uint16_t*>(residual), static_cast<uint16_t*>(y), rows, channels, p, mean, var,
+      static_cast<float>(eps), save_invstd, weight, bias, relu);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm forward kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+// b2_bn_backward_reduce (z and dy_out null; dy is the gradient) and b2_bn_backward_reduce_relu (relu: dy is dz).
+int bn_backward_reduce(const char* fn, bool relu, const void* dy, const void* z, const void* x, void* dy_out, size_t rows, size_t channels,
+                       int dtype, const float* mean, const float* invstd, float* sum_dy, float* sum_dy_xmu, float* grad_weight,
+                       float* grad_bias, void* workspace, size_t workspace_bytes, int device, void* stream) {
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
+  if (relu) {
+    if (const int rc = bn_check_ptrs(fn, {{"dz", dy, 16}, {"z", z, 16}, {"x", x, 16}, {"dy", dy_out, 16}})) return rc;
+  } else if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}})) {
+    return rc;
+  }
+  if (const int rc = bn_check_ptrs(fn, {{"mean", mean, 4}, {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4}, {"sum_dy_xmu", sum_dy_xmu, 4},
+                                        {"grad_weight", grad_weight, 4}, {"grad_bias", grad_bias, 4}}))
+    return rc;
+  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
+  const bn::Tree t = bn::tree(M, C);
+  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* ws = static_cast<float*>(workspace);
+  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
+  k_bn2d_bwd_reduce<kBnReduceUnroll><<<rg.grid, rg.block, 0, s>>>(
+      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(z), static_cast<const uint16_t*>(x), static_cast<uint16_t*>(dy_out), M, C,
+      t, rg.vw, mean, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias, ws);
+  if (t.grid_y > 1)
+    k_bn2d_bwd_reduce_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward reduce kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 int b2_bn_forward_elemt(const void* x, void* y, size_t rows, size_t channels, int dtype, const float* weight, const float* bias,
                         const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream) {
-  static const char* fn = "b2_bn_forward_elemt";
-  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
-  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"y", y, 16}, {"weight", weight, 4}, {"bias", bias, 4}, {"mean", mean, 4},
-                                        {"var", var, 4}, {"save_invstd", save_invstd, 4}}))
-    return rc;
-  DeviceGuard g(device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bn::Plan p = bn::plan(rows, channels, sm_count(device), kBnFwdUnroll);
-  // ATen converts eps to float at its launch (acc_t); so does this call
-  k_bn2d_norm<kBnFwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y), rows,
-                                                                         channels, p, mean, var, static_cast<float>(eps), save_invstd,
-                                                                         weight, bias);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm forward kernel launch: %s", cudaGetErrorString(e));
-  return B2_OK;
+  return bn_forward("b2_bn_forward_elemt", x, nullptr, y, false, rows, channels, dtype, weight, bias, mean, var, eps, save_invstd, device,
+                    stream);
+}
+
+int b2_bn_forward_relu(const void* x, const void* residual, void* y, size_t rows, size_t channels, int dtype, const float* weight,
+                       const float* bias, const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream) {
+  return bn_forward("b2_bn_forward_relu", x, residual, y, true, rows, channels, dtype, weight, bias, mean, var, eps, save_invstd, device,
+                    stream);
 }
 
 int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
@@ -2033,26 +2080,15 @@ int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* m
 int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t channels, int dtype, const float* mean, const float* invstd,
                           float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias, void* workspace, size_t workspace_bytes,
                           int device, void* stream) {
-  static const char* fn = "b2_bn_backward_reduce";
-  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
-  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
-  if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}, {"mean", mean, 4}, {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4},
-                                        {"sum_dy_xmu", sum_dy_xmu, 4}, {"grad_weight", grad_weight, 4}, {"grad_bias", grad_bias, 4}}))
-    return rc;
-  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
-  const bn::Tree t = bn::tree(M, C);
-  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
-  DeviceGuard g(device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* ws = static_cast<float*>(workspace);
-  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
-  k_bn2d_bwd_reduce<kBnReduceUnroll><<<rg.grid, rg.block, 0, s>>>(static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), M, C, t,
-                                                                 rg.vw, mean, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias, ws);
-  if (t.grid_y > 1)
-    k_bn2d_bwd_reduce_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward reduce kernel launch: %s", cudaGetErrorString(e));
-  return B2_OK;
+  return bn_backward_reduce("b2_bn_backward_reduce", false, dy, nullptr, x, nullptr, rows, channels, dtype, mean, invstd, sum_dy, sum_dy_xmu,
+                            grad_weight, grad_bias, workspace, workspace_bytes, device, stream);
+}
+
+int b2_bn_backward_reduce_relu(const void* dz, const void* z, const void* x, void* dy, size_t rows, size_t channels, int dtype,
+                               const float* mean, const float* invstd, float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias,
+                               void* workspace, size_t workspace_bytes, int device, void* stream) {
+  return bn_backward_reduce("b2_bn_backward_reduce_relu", true, dz, z, x, dy, rows, channels, dtype, mean, invstd, sum_dy, sum_dy_xmu,
+                            grad_weight, grad_bias, workspace, workspace_bytes, device, stream);
 }
 
 int b2_barrier(b2_comm_t* c, void* stream) {

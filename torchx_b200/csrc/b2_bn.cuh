@@ -7,6 +7,9 @@
 //   k_bn2d_bwd_reduce  read x, dy            sum_dy, sum_dy_xmu, grad_weight = sum_dy_xmu * invstd, grad_bias = sum_dy
 //   k_bn2d_norm        read x, write y       invstd = rsqrt(var + eps), y = w * (x - mean) * invstd + b
 //   k_bn2d_bwd_elemt   read x, dy, write dx  dx = (dy - sum_dy/M - (x - mean) * invstd^2 * sum_dy_xmu/M) * invstd * w
+// ResNet blocks fold their ReLU and residual add into two of them (b2_bn_forward_relu / b2_bn_backward_reduce_relu):
+//   k_bn2d_norm        + read residual       z = relu(bf16(bf16(y) + residual)): ATen's bf16 add_, then relu_
+//   k_bn2d_bwd_reduce  read dz, z, x, write dy  dy = threshold_backward(dz, z, 0), then the sums over dy
 // The arithmetic is that of ATen's batch_norm_collect_statistics_channels_last_kernel, batch_norm_update_stats(_and_invert),
 // batch_norm_backward_reduce_channels_last_kernel, batch_norm_transform_input_channels_last_kernel and
 // batch_norm_backward_elemt_channels_last_kernel, expression for expression and, for the reductions, in ATen's order:
@@ -70,6 +73,35 @@ __device__ __forceinline__ uint4 pack(const float (&f)[8]) {
 }
 
 __device__ __forceinline__ uint4 ld_vec(const uint16_t* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+
+// A coherent load, for data the kernel may overwrite (the fused reduce's dz, when dy_out is dz)
+__device__ __forceinline__ uint4 ld_vec_rw(const uint16_t* p) { return *reinterpret_cast<const uint4*>(p); }
+
+__device__ __forceinline__ float round_bf16(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+
+// What the fused forward does to the BatchNorm output y of one element, in the unfused composition's steps: y is stored
+// as bf16; the residual add is ATen's bf16 add_ (fp32 opmath, round to nearest even); relu is ATen's relu_, clamp_min(0)
+// on the bf16 value, which lets a NaN through.
+__device__ __forceinline__ float fuse_out(float y, bool add, float r, bool relu) {
+  float v = round_bf16(y);
+  if (add) v = round_bf16(__fadd_rn(v, r));
+  if (relu && !isnan(v)) v = fmaxf(v, 0.0f);
+  return v;
+}
+
+// threshold_backward(dz, z, 0) lane by lane on the bf16 words: +0 where z <= 0, dz elsewhere (a NaN z keeps dz).
+__device__ __forceinline__ uint4 relu_grad(const uint4& dz, const uint4& z) {
+  float fz[8];
+  unpack(z, fz);
+  uint32_t w[4] = {dz.x, dz.y, dz.z, dz.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t lo = fz[2 * k] <= 0.0f ? 0u : w[k] & 0x0000FFFFu;
+    const uint32_t hi = fz[2 * k + 1] <= 0.0f ? 0u : w[k] & 0xFFFF0000u;
+    w[k] = lo | hi;
+  }
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
 
 // The thread's vec column and row within the tile; `on` = it has a column (cw * rows can fall short of the CTA, and the
 // last column tile can be partial).
@@ -401,13 +433,50 @@ __device__ __forceinline__ void elemt_rows(const Lane& l, const Plan& p, unsigne
   }
 }
 
-// The reductions: thread (vec, ty, j) of ATen CTA row by = blockIdx.y runs its chain of state S over the S::kIn inputs
-// (in0, in1), with U rows' loads issued before the first is used; then the slot merge and the vertical merge through
-// shared memory.  With grid_y == 1 the CTA hands each vec's state to out(state, col), otherwise it writes its partial,
-// which reduce_partials folds.  `mean` feeds begin (the backward's; null for the statistics).
+// One thread's chain of state S over the S::kIn inputs (in0, in1) from `row`, with U rows' loads issued before the first is
+// used.  kMask (the backward reduce only): in0 is dz, and each row's dy = relu_grad(dz, z) is written to dy_out and summed;
+// dy_out may be dz itself (each row is read, then written, by one thread).
+template <int U, bool kMask, class S>
+__device__ __forceinline__ void chain(S& s, const float (&m)[8], const uint16_t* in0, const uint16_t* in1, const uint16_t* z,
+                                      uint16_t* dy_out, int M, int C, const Tree& t, int row, unsigned long long col) {
+  constexpr int kLoads = S::kIn + (kMask ? 1 : 0);
+  const int stride = kAtenLoads * t.seq;
+  for (int i = 0; i < t.loops; i += U) {
+    uint4 q[U][kLoads];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int r = row + u * stride;
+      const bool ld = i + u < t.loops && r < M;
+      const uint16_t* p0 = in0 + static_cast<unsigned long long>(r) * C + col;
+      q[u][0] = ld ? (kMask ? ld_vec_rw(p0) : ld_vec(p0)) : make_uint4(0, 0, 0, 0);
+      if constexpr (S::kIn == 2) q[u][1] = ld ? ld_vec(in1 + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+      if constexpr (kMask) q[u][2] = ld ? ld_vec(z + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      if (i + u < t.loops) {
+        const int r = row + u * stride;
+        if constexpr (kMask) {
+          q[u][0] = relu_grad(q[u][0], q[u][2]);
+          if (r < M) *reinterpret_cast<uint4*>(dy_out + static_cast<unsigned long long>(r) * C + col) = q[u][0];
+        }
+        float f[S::kIn][8];
+#pragma unroll
+        for (int n = 0; n < S::kIn; ++n) unpack(q[u][n], f[n]);
+        update(s, m, r < M, f);
+      }
+    }
+    row += U * stride;
+  }
+}
+
+// The reductions: thread (vec, ty, j) of ATen CTA row by = blockIdx.y runs its chain; then the slot merge and the
+// vertical merge through shared memory.  With grid_y == 1 the CTA hands each vec's state to out(state, col), otherwise it
+// writes its partial, which reduce_partials folds.  `mean` feeds begin (the backward's; null for the statistics).  A
+// non-null z (the backward reduce's) masks in0 = dz by relu_grad into dy_out.
 template <int U, class S, class Out>
 __device__ __forceinline__ void reduce_rows(const uint16_t* in0, const uint16_t* in1, int M, int C, const Tree& t, int vw, const float* mean,
-                                            float* ws, Out&& out) {
+                                            float* ws, Out&& out, const uint16_t* z = nullptr, uint16_t* dy_out = nullptr) {
   __shared__ Smem sm;
   const int tid = threadIdx.x;
   const int v = tid % vw, ty = (tid / vw) % t.block_y, j = tid / (vw * t.block_y);
@@ -419,27 +488,16 @@ __device__ __forceinline__ void reduce_rows(const uint16_t* in0, const uint16_t*
   float m[8];
   if (on) {
     begin(s, m, mean, col);
-    const int stride = kAtenLoads * t.seq;
-    int row = blockIdx.y * t.block_y + ty + j * t.seq;
-    for (int i = 0; i < t.loops; i += U) {
-      uint4 q[U][S::kIn];
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int r = row + u * stride;
-        const bool ld = i + u < t.loops && r < M;
-        q[u][0] = ld ? ld_vec(in0 + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
-        if constexpr (S::kIn == 2) q[u][1] = ld ? ld_vec(in1 + static_cast<unsigned long long>(r) * C + col) : make_uint4(0, 0, 0, 0);
+    const int row = blockIdx.y * t.block_y + ty + j * t.seq;
+    // the relu-masked chain has a third input: one row in flight keeps its loads in the registers of the plain chain's
+    if constexpr (S::kIn == 2) {
+      if (z != nullptr) {
+        chain<(U > 1 ? U / 2 : 1), true>(s, m, in0, in1, z, dy_out, M, C, t, row, col);
+      } else {
+        chain<U, false>(s, m, in0, in1, nullptr, nullptr, M, C, t, row, col);
       }
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        if (i + u < t.loops) {
-          float f[S::kIn][8];
-#pragma unroll
-          for (int n = 0; n < S::kIn; ++n) unpack(q[u][n], f[n]);
-          update(s, m, row + u * stride < M, f);
-        }
-      }
-      row += U * stride;
+    } else {
+      chain<U, false>(s, m, in0, in1, nullptr, nullptr, M, C, t, row, col);
     }
   }
   put(sm, v + vw * (ty + t.block_y * j), s);
@@ -493,12 +551,14 @@ __device__ __forceinline__ void reduce_partials(int C, const Tree& t, int vw, co
 
 // ---- forward normalise --------------------------------------------------------------------------------------------------
 // invstd = rsqrt(var + eps) (ATen's batch_norm_update_stats_and_invert), written to save_invstd by the first CTA row, and
-// y = w * (x - mean) * invstd + b in batch_norm_transform_input_channels_last_kernel's order.
+// y = w * (x - mean) * invstd + b in batch_norm_transform_input_channels_last_kernel's order.  With a residual or relu,
+// y goes through fuse_out.  A residual is a second input: its rows go U / 2 at a time, so that the x and residual loads in
+// flight fit the registers of x's alone (the plan is made for that unroll).
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
-    k_bn2d_norm(const uint16_t* __restrict__ x, uint16_t* __restrict__ y, unsigned long long M, unsigned long long C, bn::Plan p,
-                const float* __restrict__ mean, const float* __restrict__ var, float eps, float* __restrict__ save_invstd,
-                const float* __restrict__ weight, const float* __restrict__ bias) {
+    k_bn2d_norm(const uint16_t* __restrict__ x, const uint16_t* __restrict__ residual, uint16_t* __restrict__ y, unsigned long long M,
+                unsigned long long C, bn::Plan p, const float* __restrict__ mean, const float* __restrict__ var, float eps,
+                float* __restrict__ save_invstd, const float* __restrict__ weight, const float* __restrict__ bias, bool relu) {
   using namespace bn;
   const Lane l = lane(p, C);
   if (!l.on) return;
@@ -514,10 +574,23 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
 #pragma unroll
     for (int k = 0; k < 8; ++k) save_invstd[l.col + k] = is[k];
   }
-  elemt_rows<U, 1>(l, p, M, C, x, nullptr, y, [&](const float (&f)[1][8], float (&o)[8]) {
+  const auto norm = [&](float v, int k) { return w[k] * (v - m[k]) * is[k] + b[k]; };
+  if (residual != nullptr) {
+    elemt_rows<(U > 1 ? U / 2 : 1), 2>(l, p, M, C, x, residual, y, [&](const float (&f)[2][8], float (&o)[8]) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = w[k] * (f[0][k] - m[k]) * is[k] + b[k];
-  });
+      for (int k = 0; k < 8; ++k) o[k] = fuse_out(norm(f[0][k], k), true, f[1][k], relu);
+    });
+  } else if (relu) {
+    elemt_rows<U, 1>(l, p, M, C, x, nullptr, y, [&](const float (&f)[1][8], float (&o)[8]) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) o[k] = fuse_out(norm(f[0][k], k), false, 0.0f, true);
+    });
+  } else {
+    elemt_rows<U, 1>(l, p, M, C, x, nullptr, y, [&](const float (&f)[1][8], float (&o)[8]) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) o[k] = norm(f[0][k], k);
+    });
+  }
 }
 
 // ---- backward elementwise ------------------------------------------------------------------------------------------------
@@ -573,16 +646,17 @@ __global__ void __launch_bounds__(bn::kBnThreads)
 // The same tree with plain sums.  ATen's kernel returns early from threads with c_offset >= C or m_offset >= M: the first
 // only ever holds channels no valid thread reads (the vertical merge pairs threads of one threadIdx.x), and m_offset =
 // by*block_y + ty < block_y*grid_y <= M for every geometry flexible_launch_configs makes, so no valid channel is affected.
+// With z (the fused forward's output) dy is the gradient dz of z: the kernel sums threshold_backward(dz, z, 0) instead,
+// in the same order, and writes it to dy_out (every row, by the thread whose chain holds it); dy_out may be dy.
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads)
-    k_bn2d_bwd_reduce(const uint16_t* __restrict__ dy, const uint16_t* __restrict__ x, int M, int C, bn::Tree t, int vw,
-                      const float* __restrict__ mean, const float* __restrict__ invstd, float* __restrict__ sum_dy,
-                      float* __restrict__ sum_dy_xmu, float* __restrict__ grad_weight, float* __restrict__ grad_bias,
-                      float* __restrict__ ws) {
+    k_bn2d_bwd_reduce(const uint16_t* dy, const uint16_t* __restrict__ z, const uint16_t* __restrict__ x, uint16_t* dy_out, int M, int C,
+                      bn::Tree t, int vw, const float* __restrict__ mean, const float* __restrict__ invstd, float* __restrict__ sum_dy, float* __restrict__ sum_dy_xmu,
+                      float* __restrict__ grad_weight, float* __restrict__ grad_bias, float* __restrict__ ws) {
   using namespace bn;
-  reduce_rows<U, Sums>(dy, x, M, C, t, vw, mean, ws, [&](const Sums& s, unsigned long long col) {
-    reduce_out(s, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias);
-  });
+  reduce_rows<U, Sums>(
+      dy, x, M, C, t, vw, mean, ws,
+      [&](const Sums& s, unsigned long long col) { reduce_out(s, col, invstd, sum_dy, sum_dy_xmu, grad_weight, grad_bias); }, z, dy_out);
 }
 
 __global__ void __launch_bounds__(bn::kBnThreads)

@@ -225,10 +225,13 @@ class DistributedDataParallel(nn.Module):
             self._used_host = torch.zeros(len(self._params), dtype=torch.int32).pin_memory()
             self._used_event = torch.cuda.Event()
         self._hooks = [p.register_post_accumulate_grad_hook(self._on_grad_ready) for p in self._params]
-        # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen
+        # exact nn.BatchNorm2d layers run channels-last bf16 / fp16 training on native kernels, everything else on ATen;
+        # torchvision's ResNet blocks run their ReLUs and residual adds inside those kernels
         from torchx_b200.nn.bn2d import convert_batchnorm
+        from torchx_b200.nn.resnet import fuse_resnet
 
         convert_batchnorm(module)
+        fuse_resnet(module)
         self._sync_module_states()
 
     # ---- construction-time / per-forward state sync (reference: distributed.py:881-890, 2176-2243) ----
