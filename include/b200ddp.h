@@ -54,8 +54,8 @@ extern "C" {
 
 #define B2_ABI_VERSION 3 /* 3: fp16 modes B2_F32_WIRE_F16 and B2_F16; later b2_allreduce_op, b2_allgather, b2_batchnorm_stats,
                             b2_reduce_scatter, b2_bn_*_elemt, b2_alltoall*, b2_reduce_scatter_step, b2_bn_reduce_plan, b2_bn_stats,
-                            b2_bn_backward_reduce, b2_reduce, b2_reduce_scatter_step_bf16, b2_comm_create_group, b2_bn_forward_relu and
-                            b2_bn_backward_reduce_relu, which only add symbols: a binding that needs them fails to resolve them against an
+                            b2_bn_backward_reduce, b2_reduce, b2_reduce_scatter_step_bf16, b2_comm_create_group, b2_bn_forward_relu,
+                            b2_bn_backward_reduce_relu and the three SyncBatchNorm b2_bn_* passes, which only add symbols: a binding that needs them fails to resolve them against an
                             older library */
 #define B2_MAX_WORLD 8 /* one NVSwitch domain: 8 x H100 */
 
@@ -536,6 +536,28 @@ int b2_bn_forward_relu(const void* x, const void* residual, void* y, size_t rows
 int b2_bn_backward_reduce_relu(const void* dz, const void* z, const void* x, void* dy, size_t rows, size_t channels, int dtype,
                                const float* mean, const float* invstd, float* sum_dy, float* sum_dy_xmu, float* grad_weight, float* grad_bias,
                                void* workspace, size_t workspace_bytes, int device, void* stream);
+
+/*
+ * SyncBatchNorm's compute passes on the same [rows, channels] view, with the bits of torch's SyncBatchNorm function
+ * (torch.batch_norm_stats, torch.batch_norm_elemt and the count form of torch.batch_norm_backward_elemt): the same kernels
+ * as above with the differences ATen's SyncBatchNorm kernels have (DESIGN.md 2.4).  The checks are those of the calls above.
+ */
+/* mean <- the batch mean; invstd <- 1 / sqrt(var + eps) in double rounded to float (0 where var and eps are both 0), with
+ * var the biased batch variance and eps converted to float first, as ATen's InvStd.  No running statistics. */
+int b2_bn_stats_invstd(const void* x, size_t rows, size_t channels, int dtype, float* mean, float* invstd, double eps, void* workspace,
+                       size_t workspace_bytes, int device, void* stream);
+
+/* y <- weight * (x - mean) * invstd + bias with invstd as given (nothing saved); with relu (and a residual, which may be
+ * null) y <- relu(that + residual) as b2_bn_forward_relu. */
+int b2_bn_forward_invstd(const void* x, const void* residual, void* y, int relu, size_t rows, size_t channels, int dtype, const float* weight,
+                         const float* bias, const float* mean, const float* invstd, int device, void* stream);
+
+/* b2_bn_backward_elemt with 1 / rows replaced by 1 / (the sum of counts[0 .. n_counts)): every rank's count (float, truncated
+ * to int32 as torch's .to(torch.int32)), summed in int64, converted to float, then the float reciprocal.  A null counts or
+ * n_counts outside 1..B2_MAX_WORLD is B2_EINVAL. */
+int b2_bn_backward_elemt_counts(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
+                                const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, const float* counts,
+                                int n_counts, int device, void* stream);
 
 /* Device-side barrier across all ranks, ordered on `stream`. */
 int b2_barrier(b2_comm_t* comm, void* stream);

@@ -1944,14 +1944,19 @@ int bn_check_workspace(const char* fn, const void* ws, size_t have, size_t need)
   return B2_OK;
 }
 
-// b2_bn_forward_elemt (residual null, no relu) and b2_bn_forward_relu.
+// b2_bn_forward_elemt (residual null, no relu), b2_bn_forward_relu and, with `given` (var is the invstd, nothing saved),
+// b2_bn_forward_invstd.
 int bn_forward(const char* fn, const void* x, const void* residual, void* y, bool relu, size_t rows, size_t channels, int dtype,
-               const float* weight, const float* bias, const float* mean, const float* var, double eps, float* save_invstd, int device,
-               void* stream) {
+               const float* weight, const float* bias, const float* mean, const float* var, bool given, double eps, float* save_invstd,
+               int device, void* stream) {
   if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
-  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"y", y, 16}, {"weight", weight, 4}, {"bias", bias, 4}, {"mean", mean, 4},
-                                        {"var", var, 4}, {"save_invstd", save_invstd, 4}}))
+  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"y", y, 16}, {"weight", weight, 4}, {"bias", bias, 4}, {"mean", mean, 4}}))
     return rc;
+  if (given) {
+    if (const int rc = bn_check_ptrs(fn, {{"invstd", var, 4}})) return rc;
+  } else if (const int rc = bn_check_ptrs(fn, {{"var", var, 4}, {"save_invstd", save_invstd, 4}})) {
+    return rc;
+  }
   if (residual)
     if (const int rc = bn_check_ptrs(fn, {{"residual", residual, 16}})) return rc;
   DeviceGuard g(device);
@@ -1961,9 +1966,66 @@ int bn_forward(const char* fn, const void* x, const void* residual, void* y, boo
   // ATen converts eps to float at its launch (acc_t); so does this call
   k_bn2d_norm<kBnFwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(
       static_cast<const uint16_t*>(x), static_cast<const uint16_t*>(residual), static_cast<uint16_t*>(y), rows, channels, p, mean, var,
-      static_cast<float>(eps), save_invstd, weight, bias, relu);
+      static_cast<float>(eps), given ? nullptr : save_invstd, weight, bias, relu);
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm forward kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+// b2_bn_backward_elemt (1 / rows) and, with_counts, b2_bn_backward_elemt_counts (1 / the sum of the n_counts counts).
+int bn_backward_elemt(const char* fn, const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
+                      const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, bool with_counts,
+                      const float* counts, int n_counts, int device, void* stream) {
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}, {"dx", dx, 16}, {"weight", weight, 4}, {"mean", mean, 4},
+                                        {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4}, {"sum_dy_xmu", sum_dy_xmu, 4}}))
+    return rc;
+  if (with_counts) {
+    if (n_counts < 1 || n_counts > B2_MAX_WORLD)
+      return fail(B2_EINVAL, "%s: n_counts=%d must be in 1..%d", fn, n_counts, B2_MAX_WORLD);
+    if (const int rc = bn_check_ptrs(fn, {{"counts", counts, 4}})) return rc;
+  }
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bn::Plan p = bn::plan(rows, channels, sm_count(device), kBnBwdUnroll);
+  // ATen's norm_fct: 1 / count in double, converted to float (the kernel replaces it when given the counts)
+  k_bn2d_bwd_elemt<kBnBwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(
+      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), static_cast<uint16_t*>(dx), rows, channels, p, mean, invstd,
+      weight, sum_dy, sum_dy_xmu, static_cast<float>(1.0 / static_cast<double>(rows)), with_counts ? counts : nullptr, n_counts);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward kernel launch: %s", cudaGetErrorString(e));
+  return B2_OK;
+}
+
+// b2_bn_stats (var and the running statistics) and b2_bn_stats_invstd (invstd, no running statistics).
+int bn_stats(const char* fn, const void* x, size_t rows, size_t channels, int dtype, float* mean, float* var, bool invstd, float* running_mean,
+             float* running_var, double momentum, double eps, void* workspace, size_t workspace_bytes, int device, void* stream) {
+  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
+  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
+  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"mean", mean, 4}, {invstd ? "invstd" : "var", var, 4}})) return rc;
+  if ((running_mean == nullptr) != (running_var == nullptr))
+    return fail(B2_EINVAL, "%s: running_mean and running_var must both be given or both be null", fn);
+  if (running_mean)
+    if (const int rc = bn_check_ptrs(fn, {{"running_mean", running_mean, 4}, {"running_var", running_var, 4}})) return rc;
+  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
+  const bn::Tree t = bn::tree(M, C);
+  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
+  DeviceGuard g(device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // ATen's update lambda takes momentum as float and bessel = N / (N - 1) computed in double, rounded to float; its
+  // statistics kernel takes eps as float (and widens it back to double in InvStd)
+  const float mom = static_cast<float>(momentum);
+  const float bessel = static_cast<float>(static_cast<double>(rows) / static_cast<double>(rows - 1));
+  const float e32 = static_cast<float>(eps);
+  float* ws = static_cast<float*>(workspace);
+  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
+  k_bn2d_stats<kBnStatsUnroll><<<rg.grid, rg.block, 0, s>>>(static_cast<const uint16_t*>(x), M, C, t, rg.vw, mean, var, running_mean,
+                                                           running_var, mom, bessel, invstd, e32, ws);
+  if (t.grid_y > 1)
+    k_bn2d_stats_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, mean, var, running_mean, running_var, mom, bessel, invstd,
+                                                                e32);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm statistics kernel launch: %s", cudaGetErrorString(e));
   return B2_OK;
 }
 
@@ -2004,34 +2066,34 @@ extern "C" {
 
 int b2_bn_forward_elemt(const void* x, void* y, size_t rows, size_t channels, int dtype, const float* weight, const float* bias,
                         const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream) {
-  return bn_forward("b2_bn_forward_elemt", x, nullptr, y, false, rows, channels, dtype, weight, bias, mean, var, eps, save_invstd, device,
-                    stream);
+  return bn_forward("b2_bn_forward_elemt", x, nullptr, y, false, rows, channels, dtype, weight, bias, mean, var, false, eps, save_invstd,
+                    device, stream);
 }
 
 int b2_bn_forward_relu(const void* x, const void* residual, void* y, size_t rows, size_t channels, int dtype, const float* weight,
                        const float* bias, const float* mean, const float* var, double eps, float* save_invstd, int device, void* stream) {
-  return bn_forward("b2_bn_forward_relu", x, residual, y, true, rows, channels, dtype, weight, bias, mean, var, eps, save_invstd, device,
-                    stream);
+  return bn_forward("b2_bn_forward_relu", x, residual, y, true, rows, channels, dtype, weight, bias, mean, var, false, eps, save_invstd,
+                    device, stream);
+}
+
+int b2_bn_forward_invstd(const void* x, const void* residual, void* y, int relu, size_t rows, size_t channels, int dtype, const float* weight,
+                         const float* bias, const float* mean, const float* invstd, int device, void* stream) {
+  return bn_forward("b2_bn_forward_invstd", x, residual, y, relu != 0, rows, channels, dtype, weight, bias, mean,
+                    invstd, true, 0.0, nullptr, device, stream);
 }
 
 int b2_bn_backward_elemt(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
                          const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, int device,
                          void* stream) {
-  static const char* fn = "b2_bn_backward_elemt";
-  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
-  if (const int rc = bn_check_ptrs(fn, {{"dy", dy, 16}, {"x", x, 16}, {"dx", dx, 16}, {"weight", weight, 4}, {"mean", mean, 4},
-                                        {"invstd", invstd, 4}, {"sum_dy", sum_dy, 4}, {"sum_dy_xmu", sum_dy_xmu, 4}}))
-    return rc;
-  DeviceGuard g(device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bn::Plan p = bn::plan(rows, channels, sm_count(device), kBnBwdUnroll);
-  // ATen's norm_fct: 1 / count in double, converted to float
-  k_bn2d_bwd_elemt<kBnBwdUnroll><<<dim3(p.gx, p.gy), bn::kBnThreads, 0, s>>>(
-      static_cast<const uint16_t*>(dy), static_cast<const uint16_t*>(x), static_cast<uint16_t*>(dx), rows, channels, p, mean, invstd,
-      weight, sum_dy, sum_dy_xmu, static_cast<float>(1.0 / static_cast<double>(rows)));
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm backward kernel launch: %s", cudaGetErrorString(e));
-  return B2_OK;
+  return bn_backward_elemt("b2_bn_backward_elemt", dy, x, dx, rows, channels, dtype, weight, mean, invstd, sum_dy, sum_dy_xmu, false, nullptr, 0,
+                           device, stream);
+}
+
+int b2_bn_backward_elemt_counts(const void* dy, const void* x, void* dx, size_t rows, size_t channels, int dtype, const float* weight,
+                                const float* mean, const float* invstd, const float* sum_dy, const float* sum_dy_xmu, const float* counts,
+                                int n_counts, int device, void* stream) {
+  return bn_backward_elemt("b2_bn_backward_elemt_counts", dy, x, dx, rows, channels, dtype, weight, mean, invstd, sum_dy, sum_dy_xmu, true,
+                           counts, n_counts, device, stream);
 }
 
 int b2_bn_reduce_plan(size_t rows, size_t channels, int* geometry, size_t* workspace_bytes) {
@@ -2050,31 +2112,14 @@ int b2_bn_reduce_plan(size_t rows, size_t channels, int* geometry, size_t* works
 
 int b2_bn_stats(const void* x, size_t rows, size_t channels, int dtype, float* mean, float* var, float* running_mean, float* running_var,
                 double momentum, void* workspace, size_t workspace_bytes, int device, void* stream) {
-  static const char* fn = "b2_bn_stats";
-  if (const int rc = bn_check_shape(fn, dtype, rows, channels)) return rc;
-  if (const int rc = bn_check_index32(fn, rows, channels)) return rc;
-  if (const int rc = bn_check_ptrs(fn, {{"x", x, 16}, {"mean", mean, 4}, {"var", var, 4}})) return rc;
-  if ((running_mean == nullptr) != (running_var == nullptr))
-    return fail(B2_EINVAL, "%s: running_mean and running_var must both be given or both be null", fn);
-  if (running_mean)
-    if (const int rc = bn_check_ptrs(fn, {{"running_mean", running_mean, 4}, {"running_var", running_var, 4}})) return rc;
-  const int M = static_cast<int>(rows), C = static_cast<int>(channels);
-  const bn::Tree t = bn::tree(M, C);
-  if (const int rc = bn_check_workspace(fn, workspace, workspace_bytes, bn::workspace_bytes(t, C))) return rc;
-  DeviceGuard g(device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // ATen's update lambda takes momentum as float and bessel = N / (N - 1) computed in double, rounded to float
-  const float mom = static_cast<float>(momentum);
-  const float bessel = static_cast<float>(static_cast<double>(rows) / static_cast<double>(rows - 1));
-  float* ws = static_cast<float*>(workspace);
-  const bn::ReduceGrid rg = bn::reduce_grid(t, C);
-  k_bn2d_stats<kBnStatsUnroll><<<rg.grid, rg.block, 0, s>>>(static_cast<const uint16_t*>(x), M, C, t, rg.vw, mean, var, running_mean,
-                                                           running_var, mom, bessel, ws);
-  if (t.grid_y > 1)
-    k_bn2d_stats_merge<<<rg.merge_grid, rg.merge_block, 0, s>>>(C, t, rg.mw, ws, mean, var, running_mean, running_var, mom, bessel);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(B2_ECUDA, "batchnorm statistics kernel launch: %s", cudaGetErrorString(e));
-  return B2_OK;
+  return bn_stats("b2_bn_stats", x, rows, channels, dtype, mean, var, false, running_mean, running_var, momentum, 0.0, workspace,
+                  workspace_bytes, device, stream);
+}
+
+int b2_bn_stats_invstd(const void* x, size_t rows, size_t channels, int dtype, float* mean, float* invstd, double eps, void* workspace,
+                       size_t workspace_bytes, int device, void* stream) {
+  return bn_stats("b2_bn_stats_invstd", x, rows, channels, dtype, mean, invstd, true, nullptr, nullptr, 0.0, eps, workspace,
+                  workspace_bytes, device, stream);
 }
 
 int b2_bn_backward_reduce(const void* dy, const void* x, size_t rows, size_t channels, int dtype, const float* mean, const float* invstd,

@@ -7,6 +7,9 @@
 //   k_bn2d_bwd_reduce  read x, dy            sum_dy, sum_dy_xmu, grad_weight = sum_dy_xmu * invstd, grad_bias = sum_dy
 //   k_bn2d_norm        read x, write y       invstd = rsqrt(var + eps), y = w * (x - mean) * invstd + b
 //   k_bn2d_bwd_elemt   read x, dy, write dx  dx = (dy - sum_dy/M - (x - mean) * invstd^2 * sum_dy_xmu/M) * invstd * w
+// SyncBatchNorm runs the same kernels with runtime arguments for its differences (torch.batch_norm_stats,
+// batch_norm_elemt and the count form of batch_norm_backward_elemt): the statistics write invstd (ATen's InvStd) instead
+// of var, the normalise takes the merged invstd as given, and dx's 1/M comes from the ranks' counts.
 // ResNet blocks fold their ReLU and residual add into two of them (b2_bn_forward_relu / b2_bn_backward_reduce_relu):
 //   k_bn2d_norm        + read residual       z = relu(bf16(bf16(y) + residual)): ATen's bf16 add_, then relu_
 //   k_bn2d_bwd_reduce  read dz, z, x, write dy  dy = threshold_backward(dz, z, 0), then the sums over dy
@@ -369,18 +372,28 @@ __device__ __forceinline__ void vertical(Smem& sm, S& s, int v, int vw, int ty, 
   }
 }
 
+// ATen's InvStd transform of torch.batch_norm_stats: its eps parameter is a double, so var + eps, the square root and the
+// reciprocal are IEEE double operations (sm_90 SASS: F2F.F64.F32 of var and of the float eps, DADD, MUFU.RSQ64H + Newton,
+// MUFU.RCP64H + Newton), rounded to float once; 0 where var and eps are both zero.
+__device__ __forceinline__ float inv_std(float var, float eps) {
+  if (var == 0.0f && eps == 0.0f) return 0.0f;
+  return __double2float_rn(__drcp_rn(__dsqrt_rn(__dadd_rn(static_cast<double>(var), static_cast<double>(eps)))));
+}
+
 // The end of ATen's statistics kernel and of batch_norm_update_stats_and_invert's running-statistics lambda (fp32:
 // 1 - momentum by FADD, FMUL (1 - momentum) * running, FFMA x, momentum, that; bessel = M / (M - 1) in double rounded to
-// float at the launch).
+// float at the launch).  With `invstd` the second output is inv_std(var, eps) (torch.batch_norm_stats, which updates no
+// running statistics: the host passes none).
 __device__ __forceinline__ void stats_out(const Welford& w, unsigned long long col, float* __restrict__ mean, float* __restrict__ var,
-                                          float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel) {
+                                          float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel,
+                                          bool invstd, float eps) {
   const float omm = __fsub_rn(1.0f, momentum);
   const float fn = __int2float_rn(w.n);
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const float v = __fdiv_rn(w.m2n[k], fn);
     mean[col + k] = w.mean[k];
-    var[col + k] = v;
+    var[col + k] = invstd ? inv_std(v, eps) : v;
     if (running_mean != nullptr) {
       running_mean[col + k] = __fmaf_rn(w.mean[k], momentum, __fmul_rn(omm, running_mean[col + k]));
       running_var[col + k] = __fmaf_rn(__fmul_rn(v, bessel), momentum, __fmul_rn(omm, running_var[col + k]));
@@ -551,7 +564,8 @@ __device__ __forceinline__ void reduce_partials(int C, const Tree& t, int vw, co
 
 // ---- forward normalise --------------------------------------------------------------------------------------------------
 // invstd = rsqrt(var + eps) (ATen's batch_norm_update_stats_and_invert), written to save_invstd by the first CTA row, and
-// y = w * (x - mean) * invstd + b in batch_norm_transform_input_channels_last_kernel's order.  With a residual or relu,
+// y = w * (x - mean) * invstd + b in batch_norm_transform_input_channels_last_kernel's order.  A null save_invstd means
+// var already holds invstd (SyncBatchNorm's merged statistics, which torch.batch_norm_elemt reads as given).  With a residual or relu,
 // y goes through fuse_out.  A residual is a second input: its rows go U / 2 at a time, so that the x and residual loads in
 // flight fit the registers of x's alone (the plan is made for that unroll).
 template <int U>
@@ -566,11 +580,11 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     m[k] = mean[l.col + k];
-    is[k] = rsqrtf(var[l.col + k] + eps);
+    is[k] = save_invstd != nullptr ? rsqrtf(var[l.col + k] + eps) : var[l.col + k];
     w[k] = weight[l.col + k];
     b[k] = bias[l.col + k];
   }
-  if (blockIdx.y == 0 && l.r == 0) {
+  if (save_invstd != nullptr && blockIdx.y == 0 && l.r == 0) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) save_invstd[l.col + k] = is[k];
   }
@@ -594,51 +608,73 @@ __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
 }
 
 // ---- backward elementwise ------------------------------------------------------------------------------------------------
-// ATen's per-channel constants (batch_norm_backward_elemt): m_dy = sum_dy / M, f1 = invstd^2 * sum_dy_xmu / M, f2 = w * invstd.
+// ATen's per-channel constants (batch_norm_backward_elemt): m_dy = sum_dy / M, f1 = invstd^2 * sum_dy_xmu / M, f2 = w * invstd,
+// and per element dx = ((dy - m_dy) - (x - mean) * f1) * f2.  Its sm_90 SASS, whose roundings are written out here (left to
+// nvcc, the contraction follows its register allocation): f1 and f2 by FMULs; FADD x - mean; FFMA -(x - mean), f1, t;
+// FMUL f2; and t = FFMA -sum_dy, norm_fct, dy in the scalar form (BatchNorm2d), but FADD dy - m_dy with m_dy = FMUL
+// sum_dy * norm_fct in the count form (SyncBatchNorm).  With `counts` (every rank's count as float) 1 / M is that of the
+// count form: the int64 sum of the counts as int32 (torch's .to(torch.int32) truncates), converted to float, then the IEEE
+// float reciprocal (I2F.S64, MUFU.RCP + Newton); otherwise it is the host's norm_fct.
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads, bn::kBnCtasPerSm)
     k_bn2d_bwd_elemt(const uint16_t* __restrict__ dy, const uint16_t* __restrict__ x, uint16_t* __restrict__ dx, unsigned long long M,
                      unsigned long long C, bn::Plan p, const float* __restrict__ mean, const float* __restrict__ invstd,
                      const float* __restrict__ weight, const float* __restrict__ sum_dy, const float* __restrict__ sum_dy_xmu,
-                     float norm_fct) {
+                     float norm_fct, const float* __restrict__ counts, int n_counts) {
   using namespace bn;
   const Lane l = lane(p, C);
   if (!l.on) return;
+  if (counts != nullptr) {
+    long long total = 0;
+    for (int i = 0; i < n_counts; ++i) total += __float2int_rz(counts[i]);
+    norm_fct = __frcp_rn(__ll2float_rn(total));
+  }
   float m[8], mdy[8], f1[8], f2[8];
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const unsigned long long c = l.col + k;
     m[k] = mean[c];
-    mdy[k] = sum_dy[c] * norm_fct;
+    mdy[k] = counts != nullptr ? __fmul_rn(sum_dy[c], norm_fct) : sum_dy[c];  // the scalar form keeps sum_dy
     const float is = invstd[c];
-    f2[k] = weight[c] * is;
-    f1[k] = is * is * sum_dy_xmu[c] * norm_fct;
+    f2[k] = __fmul_rn(weight[c], is);
+    f1[k] = __fmul_rn(__fmul_rn(__fmul_rn(is, is), sum_dy_xmu[c]), norm_fct);
   }
-  elemt_rows<U, 2>(l, p, M, C, dy, x, dx, [&](const float (&f)[2][8], float (&o)[8]) {
+  if (counts != nullptr) {
+    elemt_rows<U, 2>(l, p, M, C, dy, x, dx, [&](const float (&f)[2][8], float (&o)[8]) {
 #pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = (f[0][k] - mdy[k] - (f[1][k] - m[k]) * f1[k]) * f2[k];
-  });
+      for (int k = 0; k < 8; ++k)
+        o[k] = __fmul_rn(__fmaf_rn(-__fsub_rn(f[1][k], m[k]), f1[k], __fsub_rn(f[0][k], mdy[k])), f2[k]);
+    });
+  } else {
+    elemt_rows<U, 2>(l, p, M, C, dy, x, dx, [&](const float (&f)[2][8], float (&o)[8]) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        o[k] = __fmul_rn(__fmaf_rn(-__fsub_rn(f[1][k], m[k]), f1[k], __fmaf_rn(-mdy[k], norm_fct, f[0][k])), f2[k]);
+    });
+  }
 }
 
 // ---- forward statistics -------------------------------------------------------------------------------------------------
 // ATen's Welford chains; the merge kernel folds the CTA rows' partials in ATen's last-block order and, like the main
-// kernel with grid_y == 1, writes mean, var = m2n / M and the running statistics.
+// kernel with grid_y == 1, writes mean, var = m2n / M (with `invstd`: inv_std(var, eps)) and the running statistics.
 template <int U>
 __global__ void __launch_bounds__(bn::kBnThreads)
     k_bn2d_stats(const uint16_t* __restrict__ x, int M, int C, bn::Tree t, int vw, float* __restrict__ mean, float* __restrict__ var,
-                 float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel, float* __restrict__ ws) {
+                 float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel, bool invstd, float eps,
+                 float* __restrict__ ws) {
   using namespace bn;
   reduce_rows<U, Welford>(x, nullptr, M, C, t, vw, nullptr, ws, [&](const Welford& w, unsigned long long col) {
-    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
+    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel, invstd, eps);
   });
 }
 
 __global__ void __launch_bounds__(bn::kBnThreads)
     k_bn2d_stats_merge(int C, bn::Tree t, int vw, const float* __restrict__ ws, float* __restrict__ mean, float* __restrict__ var,
-                       float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel) {
+                       float* __restrict__ running_mean, float* __restrict__ running_var, float momentum, float bessel, bool invstd,
+                       float eps) {
   using namespace bn;
   reduce_partials<Welford>(C, t, vw, ws, [&](const Welford& w, unsigned long long col) {
-    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel);
+    stats_out(w, col, mean, var, running_mean, running_var, momentum, bessel, invstd, eps);
   });
 }
 

@@ -159,6 +159,9 @@ SIGNATURES = {
     "b2_bn_backward_reduce": (_i, [_vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
     "b2_bn_forward_relu": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _d, _vp, _i, _vp]),
     "b2_bn_backward_reduce_relu": (_i, [_vp, _vp, _vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _i, _vp]),
+    "b2_bn_stats_invstd": (_i, [_vp, _sz, _sz, _i, _vp, _vp, _d, _vp, _sz, _i, _vp]),
+    "b2_bn_forward_invstd": (_i, [_vp, _vp, _vp, _i, _sz, _sz, _i, _vp, _vp, _vp, _vp, _i, _vp]),
+    "b2_bn_backward_elemt_counts": (_i, [_vp, _vp, _vp, _sz, _sz, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "b2_barrier": (_i, [_vp, _vp]),
     "b2_local_pass": (_i, [_vp, _sz, _i, _f, _i, _vp]),
 }

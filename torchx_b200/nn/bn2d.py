@@ -13,6 +13,9 @@ reproduce.
 the normalise and backward-reduce passes (``b2_bn_forward_relu`` / ``b2_bn_backward_reduce_relu``) with the unfused ops' bits;
 ``torchx_b200.nn.resnet`` uses it for torchvision's ResNet blocks.
 
+``torchx_b200.nn.SyncBatchNorm`` runs the same passes in their SyncBatchNorm forms (``b2_bn_stats_invstd``,
+``b2_bn_forward_invstd``, ``b2_bn_backward_elemt_counts``) around its exchanges.
+
 ``BatchNorm2d`` is ``nn.BatchNorm2d`` with the same parameters, buffers, state-dict keys and hooks; it takes the native
 path only for an input that the kernels cover exactly (``native_eligible``) and calls ``nn.BatchNorm2d.forward``
 unchanged for everything else: eval mode, fp32 or NCHW inputs, CPU tensors, non-affine layers, and every input torch
@@ -84,7 +87,7 @@ class _NativeBatchNorm(torch.autograd.Function):
         need_x, need_w, need_b = ctx.needs_input_grad[:3]
         if not (need_x or need_w or need_b):
             return None, None, None, None, None, None, None
-        dy = grad_output.contiguous(memory_format=torch.channels_last)
+        dy = _aligned(grad_output)
         n, c, h, w = x.shape
         dev = x.device
         if native_reductions(x):
@@ -155,30 +158,39 @@ class _Normalise(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, grad_output):
         x, mean, invstd, z = ctx.saved_tensors
-        n, c, h, w = x.shape
-        dev = x.device
-        if not ctx.relu:
-            dy = grad_output.contiguous(memory_format=torch.channels_last)
-        elif grad_output.is_contiguous(memory_format=torch.channels_last):
-            dz, dy = grad_output, torch.empty_like(x, memory_format=torch.channels_last)
-        else:
-            # a gradient in another layout (a mean's backward hands ResNet's last block an NCHW one) is taken into dy and
-            # masked in place: no more activation-sized tensors are alive than in the unfused ReLU's backward
-            dz = dy = grad_output.contiguous(memory_format=torch.channels_last)
-        sum_dy, sum_dy_xmu, gw, gb = (torch.empty(c, dtype=torch.float32, device=dev) for _ in range(4))
-        ws, ws_bytes = _workspace(n * h * w, c, dev)
-        if ctx.relu:
-            N.check(N.lib().b2_bn_backward_reduce_relu(dz.data_ptr(), z.data_ptr(), x.data_ptr(), dy.data_ptr(), n * h * w, c,
-                                                       N.B2_DT_BFLOAT16, mean.data_ptr(), invstd.data_ptr(), sum_dy.data_ptr(),
-                                                       sum_dy_xmu.data_ptr(), gw.data_ptr(), gb.data_ptr(), _ptr(ws), ws_bytes,
-                                                       dev.index, _stream(dev)))
-        else:
-            N.check(N.lib().b2_bn_backward_reduce(dy.data_ptr(), x.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16, mean.data_ptr(),
-                                                  invstd.data_ptr(), sum_dy.data_ptr(), sum_dy_xmu.data_ptr(), gw.data_ptr(),
-                                                  gb.data_ptr(), _ptr(ws), ws_bytes, dev.index, _stream(dev)))
+        c = x.shape[1]
+        sum_dy, sum_dy_xmu = (torch.empty(c, dtype=torch.float32, device=x.device) for _ in range(2))
+        dy, gw, gb = _normalise_backward(grad_output, x, z, mean, invstd, sum_dy, sum_dy_xmu)
         ctx.sums.append((sum_dy, sum_dy_xmu))
         need_r, need_w, need_b = ctx.needs_input_grad[1:4]
         return dy, dy if need_r else None, gw if need_w else None, gb if need_b else None, None, None, None, None, None, None
+
+
+def _normalise_backward(grad_output, x, z, mean, invstd, sum_dy, sum_dy_xmu):
+    """The backward reduce of a native normalise into sum_dy / sum_dy_xmu: (dy, grad_weight, grad_bias).  With z (the
+    output of a normalise that ran the ReLU) dy = threshold_backward(grad_output, z, 0), formed in the same pass."""
+    n, c, h, w = x.shape
+    dev = x.device
+    if z is None:
+        dy = _aligned(grad_output)
+    elif grad_output.is_contiguous(memory_format=torch.channels_last) and grad_output.data_ptr() % 16 == 0:
+        dz, dy = grad_output, torch.empty_like(x, memory_format=torch.channels_last)
+    else:
+        # a gradient in another layout (a mean's backward hands ResNet's last block an NCHW one) is taken into dy and
+        # masked in place: no more activation-sized tensors are alive than in the unfused ReLU's backward
+        dz = dy = _aligned(grad_output, copy=True)
+    gw, gb = (torch.empty(c, dtype=torch.float32, device=dev) for _ in range(2))
+    ws, ws_bytes = _workspace(n * h * w, c, dev)
+    if z is not None:
+        N.check(N.lib().b2_bn_backward_reduce_relu(dz.data_ptr(), z.data_ptr(), x.data_ptr(), dy.data_ptr(), n * h * w, c,
+                                                   N.B2_DT_BFLOAT16, mean.data_ptr(), invstd.data_ptr(), sum_dy.data_ptr(),
+                                                   sum_dy_xmu.data_ptr(), gw.data_ptr(), gb.data_ptr(), _ptr(ws), ws_bytes,
+                                                   dev.index, _stream(dev)))
+    else:
+        N.check(N.lib().b2_bn_backward_reduce(dy.data_ptr(), x.data_ptr(), n * h * w, c, N.B2_DT_BFLOAT16, mean.data_ptr(),
+                                              invstd.data_ptr(), sum_dy.data_ptr(), sum_dy_xmu.data_ptr(), gw.data_ptr(),
+                                              gb.data_ptr(), _ptr(ws), ws_bytes, dev.index, _stream(dev)))
+    return dy, gw, gb
 
 
 # ATen reduces with its channels-last kernels only under 32-bit indexing (canUse32BitIndexMath: fewer than 2^31 - 1
@@ -190,6 +202,14 @@ def native_reductions(x: torch.Tensor) -> bool:
     """True when the two reductions of an eligible input run natively (``b2_bn_stats`` / ``b2_bn_backward_reduce``): where
     ATen itself would run its channels-last kernels.  Larger inputs keep ATen's own reduction calls."""
     return x.numel() < _INDEX32_LIMIT
+
+
+def _aligned(t: torch.Tensor, copy: bool = False) -> torch.Tensor:
+    """t as the kernels read a gradient: channels-last contiguous and 16-byte aligned (a gradient can be a view that is
+    neither), copied only where it is not (always with ``copy``)."""
+    if not copy and t.is_contiguous(memory_format=torch.channels_last) and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.channels_last)
 
 
 def _ptr(t) -> int:

@@ -9,11 +9,15 @@ BatchNorm passes (``BatchNorm2d.batch_stats`` / ``normalise``, DESIGN.md 2.5).
 * ``ResNet``: the stem's bn1 + ReLU.
 
 Each is the unfused forward's result bit for bit.  A block takes its parent's forward unchanged unless it is training,
-its BatchNorms are exactly ``torchx_b200.nn.BatchNorm2d``, its ReLU is exactly ``nn.ReLU``, no hook is registered on
-those layers and no global module hook exists, and it is not traced by ``torch.compile``.  Within a fused forward, a layer
-whose input ``native_eligible`` / ``native_reductions`` refuses, or whose residual is not a bf16 channels-last tensor of
-the output's shape, runs the unfused ``relu(bn(x) [+ residual])``.  So fp16 and fp32 activations, eval mode and
-SyncBatchNorm layers compute exactly what they computed before.
+its BatchNorms are exactly ``torchx_b200.nn.BatchNorm2d`` or exactly ``torchx_b200.nn.SyncBatchNorm`` on the fabric
+(``SyncBatchNorm._fusable``), its ReLU is exactly ``nn.ReLU``, no hook is registered on those layers and no global module
+hook exists, and it is not traced by ``torch.compile``.  Within a fused forward, a ``BatchNorm2d`` (or a SyncBatchNorm at
+one rank) whose input ``native_eligible`` / ``native_reductions`` refuses runs the unfused ``relu(bn(x) [+ residual])``, and a
+layer whose residual is not a bf16 channels-last tensor of the output's shape adds it and runs the ReLU after its
+normalise.  A SyncBatchNorm over several ranks always runs as ``batch_stats`` / ``normalise``, on ATen's
+compute where its input is not eligible: whether it fuses is decided from nothing but the block, which is the same on
+every rank, so every rank issues the block's exchanges and allreduces in the same order (DESIGN.md 2.5).  So fp16 and fp32
+activations and eval mode compute exactly what they computed before.
 """
 from __future__ import annotations
 
@@ -23,6 +27,7 @@ import torch
 from torch import nn
 from torch.nn.modules import module as _module
 
+from torchx_b200.nn.batchnorm import SyncBatchNorm
 from torchx_b200.nn.bn2d import BatchNorm2d, native_eligible, native_reductions
 
 
@@ -36,17 +41,25 @@ def _fusable(block: nn.Module, bns) -> bool:
         return False
     if type(block.relu) is not nn.ReLU or _hooked(block.relu):
         return False
-    if any(type(bn) is not BatchNorm2d or _hooked(bn) for bn in bns):
+    if any(_hooked(bn) or not (type(bn) is BatchNorm2d or (type(bn) is SyncBatchNorm and bn._fusable())) for bn in bns):
         return False
     return not (_module._global_forward_hooks or _module._global_forward_pre_hooks or _module._global_backward_hooks
                 or _module._global_backward_pre_hooks)
 
 
-def _bn_relu(bn: BatchNorm2d, relu: nn.ReLU, x: torch.Tensor, residual: Optional[Callable[[], torch.Tensor]] = None) -> torch.Tensor:
+def _two_phase(bn: nn.Module, x: torch.Tensor) -> bool:
+    """Whether ``bn`` runs as ``batch_stats`` / ``normalise``: always for a SyncBatchNorm over several ranks (its collectives
+    must not depend on this rank's input), otherwise where the native kernels cover x."""
+    if type(bn) is SyncBatchNorm and bn._comm().world > 1:
+        return True
+    return native_eligible(bn, x) and native_reductions(x)
+
+
+def _bn_relu(bn: nn.Module, relu: nn.ReLU, x: torch.Tensor, residual: Optional[Callable[[], torch.Tensor]] = None) -> torch.Tensor:
     """``relu(bn(x) + residual())`` (``relu(bn(x))`` without a residual), fused where the kernels cover the inputs.  The
     residual branch runs after the BatchNorm's statistics and before its normalise, so that the autograd graph keeps the
     unfused forward's node order (``_BatchStats``)."""
-    if not (native_eligible(bn, x) and native_reductions(x)):
+    if not _two_phase(bn, x):
         out = bn(x)
         if residual is not None:
             out += residual()
